@@ -5,11 +5,12 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --steps 4 --warmup 1      # CPU reference arm (oracle port)
+    python bench.py --steps 10 --dump-outputs DIR              # + the last timed step's results as DIR/*.npy
 
 --config selects the BASELINE.json configuration (SURVEY.md 8d); the default, 2, is the one the metric is quoted on:
   2  batch 32/GPU x 600x900, fp32-faithful conv arithmetic, DETECT_MODE H             (configs[1])
   3  batch 32/GPU x 600x900 (256 on 8 GPUs), bf16 conv operands / fp32 BiLSTM           (configs[2])
-  4  batch 64 x 1200x1600, fp32-faithful, 75 000 anchors -> 12 000 into NMS              (configs[3])
+  4  batch 32 x 1200x1600, fp32-faithful, 75 000 anchors -> 12 000 into NMS              (configs[3])
   5  batch 32/GPU of mixed 600x900 / 900x600 images, DETECT_MODE O text lines            (configs[4])
 
 One "step" = one pass of the hot path (uint8 image batch -> conv stack -> BiLSTM -> heads -> proposal layer incl. sort +
@@ -18,7 +19,7 @@ NMS -> rois [-> text lines in config 5]) over one batch of synthetic images per 
   value : whole-job images/s, inputs resident in HBM, CUDA-event timed, max over ranks
   e2e   : same metric through the public streaming API with HOST buffers (pinned H2D of the uint8 images and D2H of
           the results inside the timed region; config 5 and `e2e_text_lines`: + the text-line connector on host threads)
-  roofline : algorithmic conv FLOPs / CUDA-event time of the tcgen05 conv launches (measured live through the
+  roofline : algorithmic conv FLOPs / CUDA-event time of the wgmma conv launches (measured live through the
           library's ctpn_prof_* hooks) vs MEASURED_PEAKS.json; roofline_extra: conv1_1 (HBM), BiLSTM recurrence (fp32 FMA)
   cpu_baseline : the CPU oracle (torch-CPU float32 network + numpy proposal layer, kind "port") timed on this host's
           cores on a bounded sample of the same workload; the same leg measures parity against the oracle and times the
@@ -41,16 +42,16 @@ sys.path.insert(0, PKG)
 CONFIGS = {
     2: dict(tag="configs[1]", batch=32, shapes=[(600, 900)], mode="fp32", detect="H"),
     3: dict(tag="configs[2]", batch=32, shapes=[(600, 900)], mode="bf16", detect="H"),
-    4: dict(tag="configs[3]", batch=64, shapes=[(1200, 1600)], mode="fp32", detect="H"),
+    4: dict(tag="configs[3]", batch=32, shapes=[(1200, 1600)], mode="fp32", detect="H"),
     5: dict(tag="configs[4]", batch=32, shapes=[(600, 900), (900, 600)], mode="fp32", detect="O"),
 }
 # conv arithmetic modes of the engine (planes of Engine): what one algorithmic MAC costs in bf16-rate MMA units
 MODES = {
     "bf16": dict(planes=1, units=1.0, dtype="bf16 operands, fp32 accumulate"),
-    "bf16x2": dict(planes=2, units=3.0, dtype="fp32-faithful: bf16x2 split operands (3 tcgen05 MMAs per MAC), fp32 accumulate"),
-    "f16f8": dict(planes=4, units=2.0, dtype="fp32-faithful: fp16 operands + e4m3 cross terms (1 kind::f16 + 1 kind::f8f6f4 tcgen05 MMA per 16 MACs: "
+    "bf16x2": dict(planes=2, units=3.0, dtype="fp32-faithful: bf16x2 split operands (3 wgmma MMAs per MAC), fp32 accumulate"),
+    "f16f8": dict(planes=4, units=2.0, dtype="fp32-faithful: fp16 operands + e4m3 cross terms (1 fp16 + 1 e4m3 wgmma per 16 MACs: "
                                              "2 bf16-rate units per MAC), fp32 accumulate; matmuls around the BiLSTM on bf16x2"),
-    "bf16x3": dict(planes=3, units=6.0, dtype="fp32-equivalent: bf16x3 split operands (6 tcgen05 MMAs per MAC), fp32 accumulate"),
+    "bf16x3": dict(planes=3, units=6.0, dtype="fp32-equivalent: bf16x3 split operands (6 wgmma MMAs per MAC), fp32 accumulate"),
 }
 FP32_MODE = os.environ.get("CTPN_BENCH_FP32_MODE", "f16f8")      # the float32-faithful mode configs 2/4/5 run in (bf16x2: the 3-unit one)
 VGG = [("conv1_1", 3, 64, 0), ("conv1_2", 64, 64, 1), ("conv2_1", 64, 128, 0), ("conv2_2", 128, 128, 1), ("conv3_1", 128, 256, 0),
@@ -83,11 +84,13 @@ def parse():
     ap.add_argument("--alt-modes", type=int, default=1, help="config 2 on 1 GPU: also time the bf16x2 (3-unit) and bf16 (configs[2]) arithmetic")
     ap.add_argument("--cpu-sample", type=int, default=4, help="images in the cpu_baseline sample (0: skip that leg)")
     ap.add_argument("--connector-threads", type=int, default=8)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's results (rois, counts per shape bucket) to DIR/*.npy")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle sampling during the timed region (B200_PROFILING.md recipe), every 50 ms."""
+    """nvidia-smi clocks/throttle sampling during the timed region, every 50 ms (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -146,7 +149,7 @@ def cpu_oracle_rate(n_images, shapes, detect, warmup=1):
     import numpy as np
     import torch
     from oracle import net_cpu, postproc, synth, textline
-    torch.set_num_threads(min(os.cpu_count() or 1, int(os.environ.get("CTPN_CPU_THREADS", "32"))))   # >32 threads is slower on the 128-core host
+    torch.set_num_threads(min(os.cpu_count() or 1, int(os.environ.get("CTPN_CPU_THREADS", "32"))))   # >32 threads is slower on many-core hosts
     w = synth.make_weights(0)
 
     def one(seed):
@@ -291,6 +294,22 @@ def workload(cfg, B):
             "output = %s" % (B, shapes, " (equal shares, one shape bucket each)" if len(cfg["shapes"]) > 1 else "", out))
 
 
+def dump_outputs(d, outs, shapes, per_shape, rows, rank, world):
+    """What the timed path handed its caller in the last timed step: per shape bucket the rois [B, rows, 5] (float32; rows
+    past an image's count zeroed, they are unwritten buffer) and the counts [B] (as float64)."""
+    import numpy as np
+    from ctpn_b200 import Engine
+    os.makedirs(d, exist_ok=True)
+    sfx = "" if world == 1 else "_rank%d" % rank
+    for (H, W), packed in zip(shapes, outs):
+        rois, count = Engine.unpack(packed.cpu().numpy(), per_shape, rows)
+        rois = np.array(rois, dtype=np.float32)
+        for b, c in enumerate(count):
+            rois[b, int(c):] = 0.0
+        np.save(os.path.join(d, "rois_%dx%d%s.npy" % (H, W, sfx)), rois)
+        np.save(os.path.join(d, "counts_%dx%d%s.npy" % (H, W, sfx)), count.astype(np.float64))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 def main():
     a = parse()
@@ -310,7 +329,7 @@ def main():
     if world > 1:
         # The all-gather is tiny (0.64 MB per rank and step) and overlaps the next step's persistent, all-SM conv kernels: keep its
         # kernel small (few channels) and give the compute stream scheduling priority, so the collective fills the gaps between
-        # kernels instead of holding SMs the conv CTAs are waiting for (measured on 4 GPUs, profiles/r2_multigpu.md)
+        # kernels instead of holding SMs the conv CTAs are waiting for
         os.environ.setdefault("NCCL_MAX_NCHANNELS", "2")
         os.environ.setdefault("NCCL_MIN_NCHANNELS", "1")
         dist.init_process_group("nccl", device_id=dev)
@@ -334,13 +353,15 @@ def main():
 
     gather_stream = torch.cuda.Stream(device=dev) if world > 1 else None
     inflight = []            # (packed, gathered, work) of every step of the current region: released only after the region
+    last = []                # this rank's packed results of the latest step (--dump-outputs)
 
     def step_device():
         outs = [eng.detect_packed(im, info) for im, info in zip(images, infos)]
+        last[:] = outs
         if world > 1:
             # the one collective of the path: all-gather of this step's packed results, issued asynchronously on a side stream
             # behind an event of the compute stream so that it overlaps the next step (drained before the timed region closes;
-            # measured on 2 GPUs, tools/dbg_gather.py: +0.6 ms/step, a blocking gather on the compute stream +1.0 ms/step)
+            # a blocking gather on the compute stream would serialise it with the next step's kernels)
             packed = torch.cat(outs) if len(outs) > 1 else outs[0]
             done = torch.cuda.Event()
             done.record(torch.cuda.current_stream())
@@ -394,7 +415,7 @@ def main():
     sampler = ClockSampler(local) if rank == 0 else None
     # ---- value: device-resident inputs, CUDA events ----
     # per-kernel CUDA events (ctpn_prof_*): inside the timed region at N = 1; at N > 1 they perturb the overlap of the all-gather
-    # with the next step (measured: -2 % at 2 GPUs), so the timed region runs without them and the per-kernel figures of the
+    # with the next step, so the timed region runs without them and the per-kernel figures of the
     # roofline come from a separate K-step region right after it
     prof_inside = world == 1
     N.check(N.lib.ctpn_prof_enable(1 if prof_inside else 0), "prof")
@@ -408,6 +429,8 @@ def main():
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
     del inflight[:]
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, last, shapes, per_shape, post, rank, world)
     if not prof_inside:
         N.check(N.lib.ctpn_prof_enable(1), "prof")
         for _ in range(K):
@@ -480,9 +503,9 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_tf = peaks.get("bf16_tflops_sustained", 1400.0)
-        hbm = peaks.get("hbm_gbs", 6500.0)
-        peak_src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md): 1.4 PFLOP/s sustained bf16, 6.5 TB/s HBM"
+        peak_tf = peaks.get("bf16_tflops_sustained", 989.0)
+        hbm = peaks.get("hbm_gbs", 3350.0)
+        peak_src = "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet (700 W): 989 TFLOP/s dense bf16, 3.35 TB/s HBM3"
         works = [work_per_image(H, W) for H, W in shapes]
         conv = [p for p in prof if p["kernel"].startswith("conv_tc t9")]
         gemm = [p for p in prof if p["kernel"].startswith("conv_tc t1")]
@@ -493,7 +516,7 @@ def main():
         achieved = alg_flops / (conv_ms / 1e3) / 1e12 if conv_ms > 0 else 0.0
         traffic, traffic_note = None, "no ncu capture committed for this mode/config"
         try:        # DRAM bytes of the conv launches of one step from the committed ncu --set full capture -- only if it was
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r2_conv_traffic_cfg%d_%s.json" % (a.config, mode))))   # taken from THIS code
+            tj = json.load(open(os.path.join(ROOT, "profiles", "conv_traffic_cfg%d_%s.json" % (a.config, mode))))   # taken from THIS code
             if tj.get("sources_sha256") != sources_sha256():
                 traffic_note = "committed capture is from other kernel sources (sha mismatch): not reported"
             elif tj.get("batch") == B and tj.get("launches") == int(sum(q["launches"] for q in conv)) // K:
@@ -508,7 +531,8 @@ def main():
         c11_bytes = sum(H * W * (3 + 64 * store_planes * 2) for H, W in shapes) * per_shape
         lstm_flops = sum(w["recurrent"] for w in works) * per_shape
         lstm_bytes = sum(w["cells"] * (1024 * 4 + 256 * 2 * min(store_planes, 3)) for w in works) * per_shape
-        fma_peak = 148 * 128 * 2 * (peaks.get("sm_max_mhz", 1965.0) * 1e6) / 1e12     # fp32 FMA lanes x 2 flop x max clock
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        fma_peak = sms * 128 * 2 * (peaks.get("sm_max_mhz", 1980.0) * 1e6) / 1e12     # fp32 FMA lanes x 2 flop x max clock
         line = {
             "metric": metric_name(cfg), "value": value, "unit": "images/s", "n_gpus": world, "steps": K, "warmup": W_,
             "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -516,14 +540,14 @@ def main():
             "config": {"workload": workload(cfg, B), "baseline_config": "BASELINE.json %s (--config %d)" % (cfg["tag"], a.config),
                        "global_batch": world * B, "mode": mode, "planes": M["planes"], "streams": a.streams,
                        "parallelism": "dp%d (independent image shards, one NCCL all-gather of the packed results per batch)" % world,
-                       "l2": "no explicit flush: every step streams >4 GB of activations through the 126 MB L2, nothing survives between steps"},
+                       "l2": "no explicit flush: every step streams >4 GB of activations through the 50 MB L2, nothing survives between steps"},
             "e2e": {"value": world * B * K / e2e_s, "unit": "images/s",
                     "h2d_bytes_per_step": sum(per_shape * H * W * 3 + per_shape * 12 for H, W in shapes),
                     "d2h_bytes_per_step": B * post * 5 * 4 + B * 4,
                     "api": "Engine.detect_lines_batches (rois -> host connector threads)" if cfg["detect"] == "O" else "Engine.rois_batches"},
             "gpu_launches": int(sum(p["launches"] for p in prof)) + K * len(shapes) * 6,   # + split_heads + decode/sort/nms/compact/emit
             "clocks": clocks,
-            "roofline": {"bound": "tensor", "kernel": "conv_tc_kernel (%d tcgen05 3x3 conv launches per step)" % (len(conv) and int(sum(p["launches"] for p in conv)) // K),
+            "roofline": {"bound": "tensor", "kernel": "conv_tc_kernel (%d wgmma 3x3 conv launches per step)" % (len(conv) and int(sum(p["launches"] for p in conv)) // K),
                          "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic,
                          "traffic_note": traffic_note, "peak_source": peak_src + " bf16_tflops_sustained", "ms_per_step": conv_ms,
                          "measured_in": "the timed region" if world == 1 else "a separate %d-step region after the timed one (per-kernel events perturb the all-gather overlap at N > 1)" % K,
@@ -537,7 +561,7 @@ def main():
                 {"kernel": "bilstm_kernel (recurrence)", "bound": "fp32 FMA (latency-bound in practice)", "achieved": lstm_flops / max(lstm_ms, 1e-9) / 1e9,
                  "peak": fma_peak, "unit": "TFLOP/s", "frac": lstm_flops / max(lstm_ms, 1e-9) / 1e9 / fma_peak, "ms_per_step": lstm_ms,
                  "hbm_frac": lstm_bytes / max(lstm_ms, 1e-9) / 1e6 / hbm,
-                 "note": "0.543 GFLOP/image of h.Wh at 600x900; peak = 148 SMs x 128 lanes x 2 x max SM clock; hbm_frac = (x-projection read + h write) / time / HBM peak"},
+                 "note": "0.543 GFLOP/image of h.Wh at 600x900; peak = %d SMs x 128 lanes x 2 x max SM clock; hbm_frac = (x-projection read + h write) / time / HBM peak" % sms},
             ],
             "stage_ms_per_step": dict({"conv_tc 3x3": conv_ms, "conv_tc 1x1 GEMMs": sum(p["ms"] for p in gemm) / K},
                                       **{p["kernel"]: p["ms"] / K for p in other}),

@@ -1,7 +1,7 @@
 /*
- * ctpn_b200 -- C ABI of the B200-native CTPN detection hot path.
+ * ctpn_b200 -- C ABI of the H100-native (sm_90a) CTPN detection hot path.
  *
- * One shared library (libctpn_b200.so, nvcc -gencode arch=compute_100a,code=sm_100a),
+ * One shared library (libctpn_b200.so, nvcc -gencode arch=compute_90a,code=sm_90a),
  * plain pointers and sizes only, no torch / C++ types.  Every entry point returns an
  * int status (0 = success); ctpn_last_error() gives the message for the calling thread.
  * Unless a name ends in _host, pointers are DEVICE pointers on the current device and
@@ -46,7 +46,7 @@ extern "C" {
 #define CTPN_ERR_INVALID 1   /* bad argument */
 #define CTPN_ERR_CUDA 2      /* CUDA runtime / driver error */
 #define CTPN_ERR_WORKSPACE 3 /* workspace too small */
-#define CTPN_ERR_NO_DEVICE 4 /* no usable sm_100 device */
+#define CTPN_ERR_NO_DEVICE 4 /* no usable sm_90 device */
 
 /* ---- library ------------------------------------------------------------------------- */
 int ctpn_version(void);                 /* 10000*major + 100*minor + patch */
@@ -98,7 +98,7 @@ int ctpn_proposals(const float *cls, int cls_is_logit, const float *bbox, const 
  * Activation format ("planes"): P in {1,2,3} bf16 tensors [P][B][H][W][C] whose element-wise
  * sum is the float32 value (a = a1 + a2 (+ a3), a1 = bf16(a), a2 = bf16(a - a1), ...).
  * P=1 is plain bf16, P=3 carries all 24 mantissa bits.  Products of planes are accumulated
- * in float32 on the tensor cores (tcgen05, TMEM accumulators).
+ * in float32 on the tensor cores (wgmma, register accumulators).
  * Weight format: bf16 [P][Cout][taps][Cin] (K-major), made by ctpn_pack_weights from the
  * TF layout [taps][Cin][Cout] (HWIO for 3x3, [K][N] for matmuls). */
 int ctpn_pack_weights(const float *w_tf, int taps, int cin, int cout, int cout_pad, int planes,
@@ -107,11 +107,11 @@ int ctpn_pack_weights(const float *w_tf, int taps, int cin, int cout, int cout_p
 /* conv1_1: uint8 BGR image [B][H][W][3] (or float32 blob when src_is_f32) -> 64-channel planes; fuses the mean
  * subtraction of lib/fast_rcnn/test.py:9 (lut[256][3] = float32(double(v) - PIXEL_MEANS[c])), bias and ReLU.  On the
  * tensor cores: the im2col tile (K = 27 padded to 32) is built in shared memory as bf16 planes and multiplied by the
- * resident weight tile with tcgen05.mma; HBM-write bound. */
+ * resident weight tile with wgmma; HBM-write bound. */
 int ctpn_conv1_1_tc(const void *src, int src_is_f32, const float *lut, const float *w_hwio,
                     const float *bias, void *out_planes, int B, int H, int W, int planes, void *stream);
 
-/* 3x3 SAME conv (taps=9) or 1x1 / matmul (taps=1) on planes with tcgen05 tensor cores.
+/* 3x3 SAME conv (taps=9) or 1x1 / matmul (taps=1) on planes with wgmma tensor cores.
  * flags: bit0 ReLU, bit1 fused 2x2/2 VALID max-pool (taps=9 only), bit2 float32 output
  * [B][H][W][Cout] instead of planes.  Cin % 64 == 0, Cout % 64 == 0. */
 #define CTPN_F_RELU 1
@@ -127,8 +127,8 @@ int ctpn_conv1_1_tc(const void *src, int src_is_f32, const float *lut, const flo
 int ctpn_conv3x3(const void *in_planes, const void *w_planes, const float *bias, void *out, int B,
                  int H, int W, int cin, int cout, int taps, int planes, int flags, void *stream);
 /* The same layers in the "F16F8" arithmetic: 2 tensor-core units per MAC instead of the 3 of two bf16 planes; head logits
- * within 1e-3 of float32, 6-8e-4 measured (DESIGN.md section 5).  A value a is carried as h = fp16(a * s) plus e4m3 copies of a and of the exact
- * residual a * s - h; products are h_a * h_w on kind::f16 MMAs plus the two cross terms on kind::f8f6f4 MMAs.
+ * within 1e-3 of float32 (DESIGN.md section 5).  A value a is carried as h = fp16(a * s) plus e4m3 copies of a and of the exact
+ * residual a * s - h; products are h_a * h_w on fp16 MMAs plus the two cross terms on e4m3 MMAs.
  * Activation planes: [0] fp16 [B][H][W][C]; [1] per pixel and 64-channel block 128 bytes e4m3(a * t)[64] | e4m3(r * 2^11 t / s)[64].
  * Weight planes (ctpn_pack_weights_f16f8): [0] fp16(w * s_w) [Cout][taps][Cin]; [1] per (cout, tap, 64-channel block)
  * e4m3(r_w * 2^11 t_w / s_w)[64] | e4m3(w * t_w)[64].  All scales are powers of two chosen by the caller (per tensor).

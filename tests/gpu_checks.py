@@ -287,7 +287,7 @@ def cmd_bilstm(a):
 
 
 def cmd_net_simt(a):
-    """Whole network, tcgen05 kernels vs the float32 SIMT reference kernels of the test library (same planes)."""
+    """Whole network, tensor-core kernels vs the float32 SIMT reference kernels of the test library (same planes)."""
     import torch
     from ctpn_b200 import Engine
     from oracle import synth

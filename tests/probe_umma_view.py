@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Hardware probe (run on the GPU box): can a UMMA A-operand descriptor address a SHIFTED view of a
+"""Hardware probe (run on the GPU box): can a wgmma A-operand descriptor address a SHIFTED view of a
 swizzled shared-memory matrix (start row not a multiple of 8, arbitrary stride between 8-row groups)?
 Prints one line per configuration; 'abs-ok' means the tensor core read row  row0 + (m//8)*stride + m%8
 and column n for every (m, n), i.e. the swizzle is a function of the absolute shared-memory address."""

@@ -34,7 +34,7 @@ def test_product_library_has_no_test_only_symbols_and_debug_library_has_them():
     hdr = open(os.path.join(ROOT, "text-detection-ctpn_b200", "csrc", "testing", "ctpn_b200_testing.h")).read()
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
     test_only = sorted(set(re.findall(r"\b(ctpn_[a-z0-9_]+)\s*\(", hdr)))
-    assert sorted(N.TESTING_SIGNATURES) == test_only and len(test_only) >= 6
+    assert sorted(N.TESTING_SIGNATURES) == test_only and len(test_only) >= 3
     dbg = C.CDLL(os.path.join(ROOT, "tests", "_native", "libctpn_b200_dbg.so"))
     for n in test_only:
         assert not hasattr(N.lib, n), "product library exports test-only symbol %s" % n

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM convolution (ctpn_conv3x3) and the float32 SIMT reference
+"""GPU: the wgmma implicit-GEMM convolution (ctpn_conv3x3) and the float32 SIMT reference
 (ctpn_conv3x3_simt) against a float64 torch conv2d evaluated on exactly the operand values the
 bf16 planes carry.  Each case runs in its own process (tests/gpu_checks.py) with a timeout so a
 faulting kernel fails one test instead of the session."""
@@ -35,7 +35,7 @@ def conv_args(B, H, W, cin, cout, taps, planes, flags, impl="tc", seed=0):
 
 # (B, H, W, cin, cout, taps, planes, flags)
 TC_CASES = [
-    (1, 1, 128, 64, 64, 1, 1, F32),            # one tile, one k-block: the minimal tcgen05 round trip
+    (1, 1, 128, 64, 64, 1, 1, F32),            # one tile, one k-block: the minimal tensor-core round trip
     (1, 1, 128, 64, 64, 1, 1, 0),              # bf16 plane output
     (1, 1, 300, 256, 128, 1, 2, F32),          # 1x1 GEMM, ragged M, several k-blocks, 3 plane pairs
     (1, 8, 16, 64, 64, 9, 1, RELU | F32),      # one 8x16 patch, all 9 taps, zero halo on every side

@@ -1,6 +1,6 @@
 """GPU: the whole engine against the CPU oracle (oracle/net_cpu.py + oracle/postproc.py) on the same
 seeded synthetic weights and images: layer-by-layer activations, head tensors, proposals through
-the reference-named API (get_network / Session / test_ctpn), batching, and the SIMT-vs-tcgen05
+the reference-named API (get_network / Session / test_ctpn), batching, and the SIMT-vs-tensor-core
 cross-check.  Floating-point tolerance: north_star's 1e-3, judged as |a-b| <= 1e-3*max(1,|b|);
 the tighter per-mode bounds asserted here are the measured behaviour of each plane count."""
 import numpy as np
@@ -80,8 +80,8 @@ def rows_matched(got, want, tol=1e-3):
     return hit / float(len(want))
 
 
-# measured on B200 (profiles/r2_pytest_gpu.txt): head max|diff| cls / bbox vs the float32 oracle at 600x900:
-# bf16x2 3.3e-4 / 3.4e-5, bf16x3 2.2e-4 / 2.3e-5, f16f8 6.8e-4 / 8.4e-5; bounds = those with headroom, all inside 1e-3
+# head max|diff| cls / bbox vs the float32 oracle at 600x900, per arithmetic (planes 2 = bf16x2, 3 = bf16x3, 4 = f16f8):
+# bounds with headroom over the measured deviations, all inside 1e-3
 HEAD_BOUNDS = {2: (6e-4, 8e-5), 3: (4e-4, 6e-5), 4: (1e-3, 2e-4)}
 
 
@@ -118,7 +118,6 @@ def test_end_to_end_600x900_against_oracle(weights, planes):
     want2, _, want2_idx = postproc.proposal_layer(ref["rpn_cls_prob_reshape"], ref["rpn_bbox_pred"], info, return_index=True)
     frac, ds, db = _match_rois(got, got_idx, want2, want2_idx)
     print("planes", planes, "e2e overlap %.4f  dscore %.2e  dbox %.2e" % (frac, ds, db))
-    # measured: overlap 1.0000 in every mode, dscore <= 1.3e-6, dbox <= 4.4e-5 (relative)
     assert frac >= 0.999 and ds < 1e-5 and db < 2e-4, (frac, ds, db)
 
 
@@ -276,7 +275,7 @@ def test_batch_equals_singles_and_simt_cross_check(weights):
 
 def test_bf16_mode_measured_deviation(weights):
     """BASELINE.json configs[2] arithmetic (bf16 operands, planes=1) does NOT meet the 1e-3 bar; this pins what it does
-    deliver at 600x900 (measured on B200: head logits within 0.11, 94.8 % of the oracle's rows reproduced within 1e-3)."""
+    deliver at 600x900."""
     from ctpn_b200 import Engine
     eng = Engine(weights, planes=1)
     im = synth.make_image(7)
@@ -295,7 +294,7 @@ def test_bf16_mode_measured_deviation(weights):
 @pytest.mark.parametrize("seed", [11, 12, 13, 14, 15, 16])
 def test_f16f8_mode_head_error_over_several_images(weights, seed):
     """The 2-unit arithmetic on more images than the one of test_end_to_end: every one must stay inside the 1e-3 contract on
-    the head tensors (measured 6.8e-4 .. 7.9e-4 on the logits, < 1e-4 on the regressions) with all oracle rows reproduced."""
+    the head tensors with all oracle rows reproduced."""
     from ctpn_b200 import Engine
     eng = Engine(weights, mode="f16f8")
     im = synth.make_image(seed)

@@ -7,8 +7,8 @@
 // units: CTA r keeps the 4 x 64 gate columns of units [64r, 64r+64) (128 KiB) resident in shared
 // memory for the whole sequence and the two CTAs exchange their halves of h_t through
 // distributed shared memory once per step.  Each cluster advances RG independent rows of one
-// direction, so Wh is read from shared memory once per RG rows.  All arithmetic is float32; the mat-vec uses the
-// packed fma.rn.f32x2 of sm_100 (two k per instruction: even-k and odd-k partial sums, added at the end).
+// direction, so Wh is read from shared memory once per RG rows.  All arithmetic is float32; the mat-vec keeps even-k and
+// odd-k partial sums (added at the end) so that one 16-byte weight load feeds two k.
 //
 // TF 1.3 LSTMCell: gates (i, j, f, o) = [x, h] . kernel + bias;
 //   c = sigmoid(f + 1) * c + sigmoid(i) * tanh(j);  h = sigmoid(o) * tanh(c).
@@ -64,7 +64,7 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
   const int gcol0 = (lc0 / kUnits) * kHid + rank * kUnits + (lc0 % kUnits);   // column in the 512-wide gate vector
   const int ul = t % kUnits;
   const float *wh = dir ? wh_bw : wh_fw;
-  // Shared-memory layout of the weights for packed (f32x2) FMAs: [column pair half][k pair][column group][4] with
+  // Shared-memory layout of the weights for the paired FMAs: [column pair half][k pair][column group][4] with
   // the 4 floats = (col a: k even, k odd; col b: k even, k odd), so one LDS.128 hands a thread two (k, k+1) weight
   // pairs and consecutive lanes read consecutive 16-byte chunks (conflict-free).
   for (int i = t; i < kHid * kLocalCols; i += 256) {
@@ -95,8 +95,8 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
     const int tpos = dir ? W - 1 - step : step;
     const float *hc = hbuf + (step & 1) * RG * kHid;
     const int hn_off = ((step + 1) & 1) * RG * kHid;
-    // acc[r][c] = (sum over even k, sum over odd k) for local column lc0 + c: one FFMA2 (sm_100 fma.rn.f32x2)
-    // advances two k at once with the natural register pairs (h[k], h[k+1]) x (w[k][c], w[k+1][c]).
+    // acc[r][c] = (sum over even k, sum over odd k) for local column lc0 + c: each ffma2_rn advances two k at once with the
+    // natural register pairs (h[k], h[k+1]) x (w[k][c], w[k+1][c]).
     float2 acc[RT][4];
 #pragma unroll
     for (int r = 0; r < RT; ++r) {
@@ -122,14 +122,14 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
       for (int r = 0; r < RT; ++r) {
         const float4 h4 = *reinterpret_cast<const float4 *>(hc + (rg * RT + r) * kHid + k);
         const float2 h01 = make_float2(h4.x, h4.y), h23 = make_float2(h4.z, h4.w);
-        acc[r][0] = __ffma2_rn(h01, make_float2(wa0.x, wa0.y), acc[r][0]);
-        acc[r][1] = __ffma2_rn(h01, make_float2(wa0.z, wa0.w), acc[r][1]);
-        acc[r][2] = __ffma2_rn(h01, make_float2(wb0.x, wb0.y), acc[r][2]);
-        acc[r][3] = __ffma2_rn(h01, make_float2(wb0.z, wb0.w), acc[r][3]);
-        acc[r][0] = __ffma2_rn(h23, make_float2(wa1.x, wa1.y), acc[r][0]);
-        acc[r][1] = __ffma2_rn(h23, make_float2(wa1.z, wa1.w), acc[r][1]);
-        acc[r][2] = __ffma2_rn(h23, make_float2(wb1.x, wb1.y), acc[r][2]);
-        acc[r][3] = __ffma2_rn(h23, make_float2(wb1.z, wb1.w), acc[r][3]);
+        acc[r][0] = ffma2_rn(h01, make_float2(wa0.x, wa0.y), acc[r][0]);
+        acc[r][1] = ffma2_rn(h01, make_float2(wa0.z, wa0.w), acc[r][1]);
+        acc[r][2] = ffma2_rn(h01, make_float2(wb0.x, wb0.y), acc[r][2]);
+        acc[r][3] = ffma2_rn(h01, make_float2(wb0.z, wb0.w), acc[r][3]);
+        acc[r][0] = ffma2_rn(h23, make_float2(wa1.x, wa1.y), acc[r][0]);
+        acc[r][1] = ffma2_rn(h23, make_float2(wa1.z, wa1.w), acc[r][1]);
+        acc[r][2] = ffma2_rn(h23, make_float2(wb1.x, wb1.y), acc[r][2]);
+        acc[r][3] = ffma2_rn(h23, make_float2(wb1.z, wb1.w), acc[r][3]);
       }
     }
 #pragma unroll
@@ -195,16 +195,24 @@ extern "C" int ctpn_bilstm_recurrent(const float *xproj, const float *wh_fw, con
   CTPN_REQUIRE(R > 0 && W > 0, "ctpn_bilstm_recurrent: bad shape R=%d W=%d", R, W);
   CTPN_REQUIRE(planes >= 1 && planes <= 3, "ctpn_bilstm_recurrent: planes must be 1..3");
   cudaStream_t st = (cudaStream_t)stream;
-  // rows per cluster: as many as keeps every SM busy in a single wave (148 SMs = 74 2-CTA clusters per direction pair).
-  // The 4-CTA-cluster variant (two CTAs per SM, 16 warps) was measured SLOWER on B200 (0.93 vs 0.67 ms at R = 1184, W = 56:
-  // every row group re-reads the weight slice, so two CTAs per SM double the shared-memory traffic, and the h exchange
-  // and the cluster barrier span four CTAs); it stays selectable in the test library (CTPN_LSTM_NC=4) for that record.
+  // Rows per cluster (RG): the fewest that still run every cluster in ONE wave.  A CTA holds 130-210 KiB of shared memory,
+  // so one CTA per SM and SMs / 4 clusters per direction in a wave; a second wave would repeat all W steps, while fewer
+  // rows per cluster shorten each step.  RG = 40 (208 KiB) is the largest slice that fits; beyond 40 x SMs / 4 rows the
+  // launch takes more than one wave.  On 132 SMs, batch 32 x 600x900 (R = 1184) runs at RG = 40: 30 clusters per direction.
+  // The 4-CTA-cluster variant (two CTAs per SM, 16 warps) re-reads the weight slice once per row group, so two CTAs per SM
+  // double the shared-memory traffic, and the h exchange and the cluster barrier span four CTAs; it stays selectable in
+  // the test library (CTPN_LSTM_NC=4) for comparison.
+  int sms = 0;
+  if (int rc = current_sm_count(&sms)) return rc;
+  const int per_wave = sms / 4 > 1 ? sms / 4 : 1;                  // 2-CTA clusters of each direction in one wave
+  auto fits = [&](int rg) { return (R + rg - 1) / rg <= per_wave; };
 #ifdef CTPN_DEBUG
   static const int force_nc = [] { const char *e = getenv("CTPN_LSTM_NC"); return e ? atoi(e) : 0; }();
-  if (R >= 32 * 37 && force_nc == 4) return launch_bilstm<32, 4>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (!fits(16) && force_nc == 4) return launch_bilstm<32, 4>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
 #endif
-  if (R >= 32 * 37) return launch_bilstm<32, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  if (R >= 16 * 37) return launch_bilstm<16, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  if (R >= 8 * 37) return launch_bilstm<8, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  return launch_bilstm<4, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (fits(4)) return launch_bilstm<4, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (fits(8)) return launch_bilstm<8, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (fits(16)) return launch_bilstm<16, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (fits(32)) return launch_bilstm<32, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  return launch_bilstm<40, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
 }

@@ -1,4 +1,4 @@
-// Shared helpers for the ctpn_b200 kernels (sm_100a only).
+// Shared helpers for the ctpn_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -14,6 +14,8 @@ namespace ctpn {
 // ---- error plumbing ---------------------------------------------------------------------
 void set_error(const char *fmt, ...);
 int cuda_fail(cudaError_t e, const char *what, const char *file, int line);
+// SM count of the current device (cached per device): grid sizes follow the GPU the library runs on
+int current_sm_count(int *sms);
 
 #define CTPN_CUDA(call)                                                        \
   do {                                                                         \
@@ -84,8 +86,8 @@ __device__ __forceinline__ void split_planes2(float a, float b, uint32_t (&w)[P]
 // ---- "F16F8" operand format (2 tensor-core units per MAC instead of the 3 of two bf16 planes) -----------------------
 // A float32 value a is carried as  h = fp16_rn(a * s)  (11 significant bits) and its exact residual  r = a * s - h
 // (|r| <= 2^-11 |h|).  A product a * w = (h_a + r_a)(h_w + r_w) / (s_a s_w) is evaluated as
-//     main  = h_a * h_w                          kind::f16 MMA (fp16 x fp16, exact products, fp32 accumulate): 1 unit
-//     cross = q(h_a) * q(r_w) + q(r_a) * q(h_w)   kind::f8f6f4 MMA on e4m3 copies, K-concatenated: 2 x 1/2 unit
+//     main  = h_a * h_w                          fp16 wgmma (fp16 x fp16, exact products, fp32 accumulate): 1 unit
+//     cross = q(h_a) * q(r_w) + q(r_a) * q(h_w)   e4m3 wgmma on e4m3 copies, K-concatenated: 2 x 1/2 unit
 // (r_a * r_w ~ 2^-22 is dropped).  Storage per element: 2 B (h) + 1 B (e4m3 of a) + 1 B (e4m3 of r) = the 4 B of two bf16
 // planes.  The e4m3 copies use per-tensor power-of-two scales t (values) and 2^11 t (residuals) so that both cross
 // products carry the same scale: e4m3(a t_a) * e4m3(r_w 2^11 t_w) and e4m3(r_a 2^11 t_a) * e4m3(w t_w).
@@ -110,23 +112,29 @@ __device__ __forceinline__ uint32_t e4m3x4(float a, float b, float c, float d) {
   return (uint32_t)lo | ((uint32_t)hi << 16);
 }
 
+// two round-to-nearest float32 products / fused multiply-adds on a pair of values
+__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // four values -> their F16F8 words: two fp16x2 words (of v * s), e4m3x4 of v * t, e4m3x4 of the residuals * rs.
-// The scalings run as packed mul.rn.f32x2 (sm_100); s == 1 (no fp16 pre-scale, the usual case) skips its multiply.
+// s == 1 (no fp16 pre-scale, the usual case) skips its multiply.
 __device__ __forceinline__ void f16f8_quad(float v0, float v1, float v2, float v3, float s, float t, float rs, uint32_t &h01,
                                            uint32_t &h23, uint32_t &qv, uint32_t &qr) {
   const float2 a = make_float2(v0, v1), b = make_float2(v2, v3);
   float2 as = a, bs = b;
   if (s != 1.f) {
-    as = __fmul2_rn(a, make_float2(s, s));
-    bs = __fmul2_rn(b, make_float2(s, s));
+    as = fmul2_rn(a, make_float2(s, s));
+    bs = fmul2_rn(b, make_float2(s, s));
   }
   float2 ra, rb;
   h01 = f16x2_split(as.x, as.y, ra.x, ra.y);
   h23 = f16x2_split(bs.x, bs.y, rb.x, rb.y);
-  const float2 at = __fmul2_rn(a, make_float2(t, t)), bt = __fmul2_rn(b, make_float2(t, t));
+  const float2 at = fmul2_rn(a, make_float2(t, t)), bt = fmul2_rn(b, make_float2(t, t));
   qv = e4m3x4(at.x, at.y, bt.x, bt.y);
-  ra = __fmul2_rn(ra, make_float2(rs, rs));
-  rb = __fmul2_rn(rb, make_float2(rs, rs));
+  ra = fmul2_rn(ra, make_float2(rs, rs));
+  rb = fmul2_rn(rb, make_float2(rs, rs));
   qr = e4m3x4(ra.x, ra.y, rb.x, rb.y);
 }
 

@@ -4,15 +4,15 @@
 // 1728 FMAs per pixel and reaches only a third of that bound.  Here the im2col tile is built IN SHARED MEMORY:
 //   * 4 builder warps (thread = pixel of a 16 x 8 patch) gather the 27 mean-subtracted inputs of their pixel from a
 //     small staged image patch, split them into P bf16 planes and write one K-major 128-byte row per plane in the
-//     128B-swizzled UMMA layout (only the first 64 bytes = 32 k-values are ever read),
+//     128B-swizzled wgmma layout (only the first 64 bytes = 32 k-values are ever read),
 //   * k = 27 of the padded K = 32 carries the bias (A holds the constant 1 there), so the epilogue has no bias add,
-//   * one thread issues 2 (k-slices) x {1,3,6} (plane pairs) tcgen05.mma of shape 128 x 64 x 16 per tile against the
-//     CTA-resident weight tile (built once from the float32 HWIO weights),
-//   * 8 epilogue warps (two per TMEM lane quarter, one 32-channel half each) do bias + ReLU + plane split and store
-//     through the same shared-memory transpose as conv_tc -- the epilogue, not the MMAs, paces this layer.
-// Accumulators (main + cross, see conv_tc.cu) are double buffered in TMEM.  Each builder group owns kSPG A stages
-// (two for P <= 2), so it starts its next tile while the MMAs of the previous one are still in flight -- with one
-// stage per group the builder sat idle for the arrive -> MMA -> commit round trip (~1000 cycles) on every tile.
+//   * two consumer warpgroups issue 2 (k-slices) x {1,3,6} (plane pairs) wgmma of shape 64 x 64 x 16 each per tile
+//     against the CTA-resident weight tile (built once from the float32 HWIO weights),
+//   * the same 8 warps (thread = pixel, one 32-channel half per set of 4 warps) then do ReLU + plane split and store
+//     through a float32 staging buffer and the same shared-memory transpose as conv_tc -- the epilogue, not the MMAs,
+//     paces this layer.
+// Accumulators (main + cross, see conv_tc.cu) live in registers.  Each builder group owns kSPG A stages (two for P <= 2),
+// so it builds its next tile while the consumers are still on the previous one.
 // Numerics: operands carry P bf16 planes like every other tensor-core layer (planes=3 is float32-equivalent).
 // Reference semantics: lib/networks/network.py:160-183 (conv1_1), lib/fast_rcnn/test.py:8-9 (mean subtraction).
 #include <mutex>
@@ -29,9 +29,8 @@ namespace ctpn {
 #endif
 
 
-constexpr int kC1tThreads = 544;          // warp 0: MMA issuer / TMEM owner, warps 1-8: two builder groups, warps 9-16: epilogue
+constexpr int kC1tThreads = 512;          // warps 0-7: two builder groups, warps 8-15: two MMA + epilogue warpgroups
 constexpr int kC1tTileBytes = 128 * 128;  // one plane of the A tile (128 pixels x 128-byte rows)
-constexpr int kC1tStagePitch = 64;          // epilogue staging rows: 64 B, 16-byte chunks XOR-swizzled by (row >> 1) & 3
 constexpr int kC1tPatch = 3 * 18 * 40;     // floats per staged input patch
 
 struct Conv1TcParams {
@@ -63,27 +62,17 @@ conv1_tc_kernel(const Conv1TcParams p) {
   // (lanes = 4 tile rows x 8 tile columns) hit 32 distinct banks
   float *patch = reinterpret_cast<float *>(bsm + P * 64 * 128);
   float *lut_s = patch + 4 * kC1tPatch;                                 // [256][3] mean-subtraction table
-  uint8_t *stage_buf = reinterpret_cast<uint8_t *>(lut_s + 768);
-  uint64_t *bars = reinterpret_cast<uint64_t *>(stage_buf + 8 * 32 * kC1tStagePitch);
-  const uint32_t fullA = smem_u32(bars), emptyA = fullA + 32, tfull = fullA + 64, tempty = fullA + 80;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 12);
+  float *epi = lut_s + 768;                                             // float32 staging [2 chunks][128 pixels][32 channels]
+  uint64_t *bars = reinterpret_cast<uint64_t *>(epi + 2 * 128 * 32);
+  const uint32_t fullA = smem_u32(bars), emptyA = fullA + 32;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < 4; ++i) {
       mbar_init(fullA + 8 * i, 128);     // every builder thread arrives
-      mbar_init(emptyA + 8 * i, 1);      // tcgen05.commit
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(tfull + 8 * i, 1);
-      mbar_init(tempty + 8 * i, 8);
+      mbar_init(emptyA + 8 * i, 2);      // the two consumer warpgroups, once their MMAs have completed
     }
     fence_mbar_init();
-  }
-  constexpr uint32_t acc_cols = (P > 1 ? 2u : 1u) * 64u;
-  if (warp == 0) {
-    tmem_alloc(smem_u32(tmem_slot), 2 * acc_cols);
-    tmem_relinquish();
   }
   if (!p.src_is_f32)
     for (int i = threadIdx.x; i < 768; i += kC1tThreads) lut_s[i] = p.lut[i];
@@ -109,51 +98,14 @@ conv1_tc_kernel(const Conv1TcParams p) {
       *reinterpret_cast<uint4 *>(bsm + pl * 64 * 128 + co * 128 + ((chunk ^ (co & 7)) << 4)) = make_uint4(pk[pl][0], pk[pl][1], pk[pl][2], pk[pl][3]);
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
-    // ===== MMA issuer =====
-    constexpr uint32_t kIdesc = umma_idesc_bf16(128, 64);
-    constexpr uint32_t kHi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    int a = 0, n = 0;
-    uint32_t aph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++n) {
-      // tile n of this CTA was built by group n & 1 as its (n >> 1)-th tile
-      const int s = (n & 1) * kSPG + (n >> 1) % kSPG;
-      const uint32_t ph = (uint32_t)((n >> 1) / kSPG) & 1u;
-      mbar_wait(tempty + 8 * a, aph ^ 1u);
-      mbar_wait(fullA + 8 * s, ph);
-      tc_fence_after();
-      const uint32_t a_lo = (((a0 + s * P * kC1tTileBytes) >> 4) & 0x3FFFu) | (1u << 16);
-      const uint32_t b_lo = ((b0 >> 4) & 0x3FFFu) | (1u << 16);
-      const uint32_t d_main = tmem_base + (uint32_t)a * acc_cols, d_cross = d_main + 64;
-      if (elect_one()) {
-#pragma unroll
-        for (int i = 0; i < P; ++i)
-#pragma unroll
-          for (int j = 0; j < P - i; ++j)
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {   // K = 32 (27 real taps): two 16-wide slices
-              const uint64_t da = ((uint64_t)kHi << 32) | (a_lo + i * (kC1tTileBytes >> 4) + 2u * k);
-              const uint64_t db = ((uint64_t)kHi << 32) | (b_lo + j * ((64 * 128) >> 4) + 2u * k);
-              if (i + j == 0) mma_bf16_ss(d_main, da, db, kIdesc, k);
-              else mma_bf16_ss(d_cross, da, db, kIdesc, (k == 0 && i == 0 && j == 1) ? 0u : 1u);
-            }
-        mma_commit(emptyA + 8 * s);
-        mma_commit(tfull + 8 * a);
-      }
-      __syncwarp();
-      if (++a == 2) { a = 0; aph ^= 1u; }
-    }
-  } else if (warp <= 8) {
+  if (warp < 8) {
     // ===== im2col builders: two groups of 4 warps; group g owns stage g and builds every other tile of this CTA,
     // so two tiles are in flight and the global-load latency of the patch staging is hidden.  thread = pixel m =====
-    const int grp = (warp - 1) >> 2;
-    const int m = ((warp - 1) & 3) * 32 + lane, th = m >> 3, tw = m & 7;
+    const int grp = warp >> 2;
+    const int m = (warp & 3) * 32 + lane, th = m >> 3, tw = m & 7;
     // The raw inputs of the NEXT tile's patch pixels (this thread stages patch pixels m and m + 128 of 180) are
     // fetched into registers while the current tile is being built, so the global-load latency is off the
     // per-tile critical path of the group.
@@ -239,13 +191,22 @@ conv1_tc_kernel(const Conv1TcParams p) {
       mbar_arrive(fullA + 8 * s);
     }
   } else {
-    // ===== epilogue warps 9..16 (TMEM lane quarter = warp & 3; warps 9-12 take channels 0-31, 13-16 channels 32-63) =====
-    const int quarter = warp & 3;
+    // ===== consumers: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64) against the 64 output channels; then the
+    // epilogue with thread = pixel m (warps 8-11 take channels 0-31, 12-15 channels 32-63) =====
+    const int wg = (warp >> 2) - 2;
+    const int cw = warp - 8, chunk = cw >> 2, quarter = cw & 3;
     const int m = quarter * 32 + lane, th = m >> 3, tw = m & 7;
-    uint4 *stage_w = reinterpret_cast<uint4 *>(stage_buf + (warp - 9) * 32 * kC1tStagePitch);
-    int a = 0;
-    uint32_t aph = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // accumulator fragment rows frow, frow + 8
+    constexpr uint32_t kHi = gmma_desc_hi(1024);
+    const uint32_t b_lo = gmma_desc_lo(b0);
+    float accm[32], accc[32];
+    // the warp's own 32 staging rows double as its store-transpose block once they have been read
+    uint4 *stage_w = reinterpret_cast<uint4 *>(epi + chunk * 4096 + quarter * 1024);
+    int n = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++n) {
+      // tile n of this CTA was built by group n & 1 as its (n >> 1)-th tile
+      const int s = (n & 1) * kSPG + (n >> 1) % kSPG;
+      const uint32_t ph = (uint32_t)((n >> 1) / kSPG) & 1u;
       const unsigned b = (unsigned)tile / (unsigned)tiles_per_img, r = (unsigned)tile % (unsigned)tiles_per_img;
       const int y = (int)(r / (unsigned)p.tiles_x) * 16 + th, x = (int)(r % (unsigned)p.tiles_x) * 8 + tw;
       const bool ok = y < p.H && x < p.W;
@@ -258,24 +219,47 @@ conv1_tc_kernel(const Conv1TcParams p) {
         const unsigned lo = __shfl_sync(0xffffffffu, (unsigned)(pix & 0xffffffffll), it * 8 + (lane >> 2));
         spix[it] = (hi << 32) | lo;
       }
-      mbar_wait(tfull + 8 * a, aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)a * acc_cols;
+      mbar_wait(fullA + 8 * s, ph);
+      const uint32_t a_lo = gmma_desc_lo(a0 + s * P * kC1tTileBytes + wg * 64 * 128);
+      wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < P; ++i)
+#pragma unroll
+        for (int j = 0; j < P - i; ++j)
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {   // K = 32 (27 real taps): two 16-wide slices
+            const uint64_t da = ((uint64_t)kHi << 32) | (a_lo + i * (kC1tTileBytes >> 4) + 2u * k);
+            const uint64_t db = ((uint64_t)kHi << 32) | (b_lo + j * ((64 * 128) >> 4) + 2u * k);
+            if (i + j == 0) wgmma_bf16(accm, da, db, (uint32_t)k);
+            else wgmma_bf16(accc, da, db, (k == 0 && i == 0 && j == 1) ? 0u : 1u);
+          }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(accm);
+      if (P > 1) wgmma_fence_regs(accc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(emptyA + 8 * s);
+      if (P > 1) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) accm[i] = accm[i] + accc[i];
+      }
+      named_sync(3, 256);             // the previous tile's staging rows have been read and stored
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int q = 2 * (j & 3) + ((lane & 3) >> 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frow + 8 * h;
+          *reinterpret_cast<float2 *>(epi + (j >> 2) * 4096 + row * 32 + ((q ^ (row & 7)) << 2) + 2 * (lane & 1)) =
+              make_float2(accm[4 * j + 2 * h], accm[4 * j + 2 * h + 1]);
+        }
+      }
+      named_sync(3, 256);
       if (!C1_DBG(p, 8)) {
-        const int chunk = (warp - 9) >> 2;
-        uint32_t rr[32];
-        tmem_ld_32x32(taddr + chunk * 32, rr);
-        tmem_ld_wait();
         float v[32];
-        if (P > 1) {
-          uint32_t rc[32];
-          tmem_ld_32x32(taddr + 64 + chunk * 32, rc);
-          tmem_ld_wait();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]) + __uint_as_float(rc[i]);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]);
+        for (int q = 0; q < 8; ++q) {
+          const float4 t = *reinterpret_cast<const float4 *>(epi + chunk * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
+          v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
         }
         // the bias came in through the tensor core (k = 27 row of the weight tile x the builders' constant 1)
         if (OUTQ) {
@@ -332,24 +316,14 @@ conv1_tc_kernel(const Conv1TcParams p) {
         }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty + 8 * a);
-      if (++a == 2) { a = 0; aph ^= 1u; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * acc_cols);
   }
 }
 
 template <int P, int OUTQ = 0>
 static int launch_conv1_tc(Conv1TcParams &p, cudaStream_t st) {
-  const size_t smem = 1024 + (size_t)(P <= 2 ? 4 : 2) * P * kC1tTileBytes + (size_t)P * 64 * 128 + (4 * kC1tPatch + 768) * sizeof(float) +
-                      8 * 32 * kC1tStagePitch + 96 + 16;
+  const size_t smem = 1024 + (size_t)(P <= 2 ? 4 : 2) * P * kC1tTileBytes + (size_t)P * 64 * 128 +
+                      (4 * kC1tPatch + 768 + 2 * 128 * 32) * sizeof(float) + 64;
   constexpr int kMaxDevices = 64;
   static std::mutex mu;
   static int sm_count[kMaxDevices];      // per device: SM count (0 = attribute not set yet)

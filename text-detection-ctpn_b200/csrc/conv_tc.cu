@@ -1,28 +1,30 @@
-// 3x3 SAME convolution / 1x1 matmul on bf16 "planes" with 5th-generation tensor cores.
+// 3x3 SAME convolution / 1x1 matmul on bf16 "planes" with Hopper warpgroup MMAs (wgmma).
 //
 // Implicit GEMM: M = 128 output pixels (a 16 x 8 patch of one image per CTA tile), N = BN output
 // channels, K = taps * Cin in blocks of 64 channels.
 //   * A operand: per channel block ONE 4-D TMA box load brings the (16+2) x (8+2) x 64 halo patch of the
 //     NHWC input into shared memory (128-byte swizzle; out-of-image elements are zero-filled by the TMA
 //     unit = SAME padding and ragged edges for free).  The nine filter taps are then served as nine
-//     shifted VIEWS of that one patch: the UMMA shared-memory descriptor starts at halo row
+//     shifted VIEWS of that one patch: the wgmma shared-memory descriptor starts at halo row
 //     (ky * 10 + kx) and steps 10 rows between its 8-row groups (tile row th <-> halo row th + ky).  The
 //     tensor core applies the 128B swizzle to the absolute shared-memory address, so un-aligned views of
-//     a TMA-written buffer are consistent (verified by tests/probe_umma_view.py on B200).  This cuts the
+//     a TMA-written buffer are consistent (checked by tests/probe_umma_view.py).  This cuts the
 //     L2 -> SM traffic of A by 6.4x compared with one TMA load per tap.
 //   * B operand: weights [P][Cout][taps][Cin] viewed as a 2-D K-major matrix, one 2-D TMA box per
 //     (tap, channel block), in its own ring of stages.
-//   * D: float32 accumulators in TMEM; tcgen05.mma issued by one thread, completion via tcgen05.commit.
+//   * D: float32 accumulators in registers.  Two consumer warpgroups each own 64 of the 128 pixel rows (m64nBNk16
+//     wgmma, or k32 for e4m3) and keep one group of MMAs in flight; a stage is released when its group completes.
 //     With P > 1 planes the plane-0 x plane-0 products go to a "main" accumulator and all cross-plane
 //     products to a second one (the tensor core truncates when adding into float32; see DESIGN.md).
-//   * epilogue (2 x 4 warps; a set covers the 128 TMEM lanes and takes every other 32-column chunk): tcgen05.ld ->
-//     (+cross) -> +bias -> ReLU -> optional fused 2x2 max-pool (warp shuffles: the window of a pixel lives in lanes
-//     l, l^1, l^8, l^9) -> re-split into planes (cvt.rn.bf16x2.f32) -> transpose through swizzled shared memory ->
-//     16-byte stores that cover one pixel's 64 contiguous bytes with 4 lanes (or float32 output).
+//   * epilogue (both consumer warpgroups; thread = pixel, a set of 4 warps takes every other 32-column chunk): the
+//     accumulator fragments go through a float32 staging buffer -> +bias -> ReLU -> optional fused 2x2 max-pool (warp
+//     shuffles: the window of a pixel lives in lanes l, l^1, l^8, l^9) -> re-split into planes (cvt.rn.bf16x2.f32) ->
+//     transpose through swizzled shared memory -> 16-byte stores that cover one pixel's 64 contiguous bytes with 4 lanes
+//     (or float32 output).
 // 3x3 layers run as 2-CTA clusters that share every weight tile by TMA multicast (template parameter MC; CTPN_TC_MCAST=0
-// selects the single-CTA variant): -2.4 % (bf16x2) / -2.8 % (bf16) conv time in a same-box A/B.
-// Persistent CTAs (one per SM), warp-specialised: warp 0 weight (B) producer, warp 1 MMA issuer + TMEM
-// owner, warps 2-5 and 7-10 epilogue, warp 6 activation (A) producer.  Reference: lib/networks/network.py:160-196.
+// selects the single-CTA variant).
+// Persistent CTAs (one per SM), warp-specialised: warp 0 weight (B) producer, warp 1 activation (A) producer,
+// warpgroups 1 and 2 MMAs + epilogue.  Reference: lib/networks/network.py:160-196.
 #include <cuda.h>
 
 #include <algorithm>
@@ -51,12 +53,11 @@ struct ConvTcParams {
   int PW;                   // halo patch width in pixels (= shared-memory rows per patch row)
   int patch_bytes;          // bytes of one plane's patch slot (1024-aligned)
   int patch_tx_bytes;       // bytes the TMA box actually transfers per plane
-  int group_stride_bytes;   // UMMA stride between 8-row groups of the A view
+  int group_stride_bytes;   // wgmma stride between 8-row groups of the A view
   int cout_pad;
   int Ho, Wo;
   int stages_a, stages_b;
   int debug;                // test library only (CTPN_TC_DEBUG bits): 1 skip B loads, 2 skip A loads, 4 skip MMAs, 8 skip stores
-  int nbuf;                 // TMEM tile buffers: 2 = epilogue overlaps the next tile's MMAs, 1 = serialised
   const float *bias;
   void *out;
   long long out_plane_stride;   // elements between output planes
@@ -69,32 +70,22 @@ struct ConvTcParams {
   // plain); out_rows = rows per image of the OUTPUT frame (Ho, or Ho + 1 when the output is stacked too).
   int in_stack_h, out_rows, out_stacked;
   double work;              // algorithmic FLOPs of the call (profiling label only)
-  int stage_small;          // 1: 512-byte staging block per epilogue warp (8 pixels per round) -- frees room for a 4th weight stage
+  int stage_small;          // 1: 512-byte store-transpose block per epilogue warp (8 pixels per round)
 };
 
-constexpr int kTcThreads = 352;   // warps: 0 B-producer, 1 MMA, 2-5 epilogue set 0, 6 A-producer, 7-10 epilogue set 1
+constexpr int kTcThreads = 384;   // warpgroup 0: producers (warp 0 weights, warp 1 activations); 1 and 2: MMAs + epilogue
 constexpr int kMaxStages = 8;
-constexpr int kCtrlBytes = 8 * (4 * kMaxStages + 4) + 16;
-constexpr int kStagePitch = 64;                    // bytes per pixel row of the epilogue staging buffer; 16-B chunks are
+constexpr int kCtrlBytes = 8 * (4 * kMaxStages) + 16;
+constexpr int kStagePitch = 64;                    // bytes per pixel row of the epilogue store staging; 16-B chunks are
                                                    // XOR-swizzled by (row >> 1) & 3: conflict-free writes AND reads
-constexpr int kStageBytes = 8 * 32 * kStagePitch;  // one 32-pixel x 32-channel bf16 block per epilogue warp
-
-__device__ __forceinline__ uint64_t umma_desc_a_view(uint32_t smem_addr, uint32_t group_stride_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(group_stride_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
+constexpr int kEpiBytes = 2 * 128 * 32 * 4;        // float32 staging of two 32-channel chunks of the 128-pixel tile
 
 // MC = 1: launched as 2-CTA clusters.  The two CTAs of a cluster work on two pixel tiles of the SAME output-channel tile in
 // lock step; each loads half of every weight (B) tile and TMA-multicasts it into both CTAs' shared memory, which halves the
-// L2 -> SM weight traffic (86 % of the kernel's L2 reads).  A weight stage is free when BOTH CTAs' MMAs have read it, so
-// its 'empty' barrier counts two multicast tcgen05.commit arrivals.
-// F8 = 1 (with P = 2 stage slots): the F16F8 arithmetic -- plane 0 holds fp16 operands (kind::f16 MMAs into the main
-// accumulator), plane 1 the K-concatenated e4m3 copies (kind::f8f6f4 MMAs, K = 32, into the cross accumulator): 4 + 4 tensor
+// L2 -> SM weight traffic.  A weight stage is free when BOTH CTAs' MMAs have read it, so its 'empty' barrier counts the
+// arrivals of the two consumer warpgroups of each CTA.
+// F8 = 1 (with P = 2 stage slots): the F16F8 arithmetic -- plane 0 holds fp16 operands (fp16 wgmma into the main
+// accumulator), plane 1 the K-concatenated e4m3 copies (e4m3 wgmma, K = 32, into the cross accumulator): 4 + 4 tensor
 // core instructions per (tap, channel block) where two bf16 planes need 12.
 template <int BN, int P, int TAPS, int MC, int F8>
 __global__ void __launch_bounds__(kTcThreads, 1)
@@ -103,49 +94,33 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   using namespace ptx;
   constexpr int kBBytes = BN * 128;
   static_assert(!F8 || P == 2, "F16F8 uses two stage slots per operand");
-  constexpr uint32_t kIdesc = F8 ? umma_idesc_f16(128, BN) : umma_idesc_bf16(128, BN);
-  constexpr uint32_t kIdesc8 = umma_idesc_e4m3(128, BN);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t ring_a = (raw + 1023u) & ~1023u;
   const uint32_t a_stage = (uint32_t)P * p.patch_bytes, b_stage = (uint32_t)P * kBBytes;
   const uint32_t ring_b = ring_a + (uint32_t)p.stages_a * a_stage;
-  uint8_t *stage_buf = smem_raw + (ring_b - raw) + (size_t)p.stages_b * b_stage;   // epilogue store staging
-  uint8_t *ctrl = stage_buf + (p.stage_small ? kStageBytes / 4 : kStageBytes);
+  float *epi = reinterpret_cast<float *>(smem_raw + (ring_b - raw) + (size_t)p.stages_b * b_stage);
+  uint8_t *ctrl = reinterpret_cast<uint8_t *>(epi) + kEpiBytes;
   const uint32_t fullA = smem_u32(ctrl), emptyA = fullA + 8 * kMaxStages;
   const uint32_t fullB = emptyA + 8 * kMaxStages, emptyB = fullB + 8 * kMaxStages;
-  const uint32_t tfull0 = emptyB + 8 * kMaxStages, tempty0 = tfull0 + 16;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(ctrl + 8 * (4 * kMaxStages + 4));
 
   // warp index through a shuffle so the compiler knows it is warp-uniform: the role loops below are executed by
   // whole warps with uniform control flow and only the instruction issue is predicated on one elected lane --
-  // otherwise every TMA / tcgen05 instruction gets wrapped in a per-lane 'waterfall' loop (3x slower issue).
+  // otherwise every TMA instruction gets wrapped in a per-lane 'waterfall' loop.
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     for (int s = 0; s < kMaxStages; ++s) {
       mbar_init(fullA + 8 * s, 1);
-      mbar_init(emptyA + 8 * s, 1);
+      mbar_init(emptyA + 8 * s, 2);             // the two consumer warpgroups
       mbar_init(fullB + 8 * s, 1);
-      mbar_init(emptyB + 8 * s, MC ? 2 : 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 8);
+      mbar_init(emptyB + 8 * s, MC ? 4 : 2);    // ... of each CTA of the cluster
     }
     fence_mbar_init();
   }
-  const uint32_t acc_cols = (P > 1 ? 2u : 1u) * BN;   // main (+ cross) accumulator columns per tile buffer
-  if (warp == 1) {
-    tmem_alloc(smem_u32(tmem_slot), (uint32_t)p.nbuf * acc_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
   if (MC) cluster_sync_all();      // the peer's barriers are initialised before anything is multicast into them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t rank = MC ? cluster_ctarank() : 0u;
   // persistent loop over work units: a tile, or (MC) a pair of pixel tiles x one channel tile shared by the cluster
   const int u_begin = MC ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, u_step = MC ? (int)(gridDim.x >> 1) : (int)gridDim.x;
@@ -159,8 +134,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   constexpr int halo = TAPS == 9 ? 1 : 0;
 
-  if (warp == 6) {
-    {
+  if (warp < 4) {
+    regs_dealloc<40>();
+    if (warp == 1) {
       // ===== activation (A) producer: one halo patch per plane per channel block =====
       int s = 0;
       uint32_t ph = 0;
@@ -183,9 +159,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           if (++s == p.stages_a) { s = 0; ph ^= 1u; }
         }
       }
-    }
-  } else if (warp == 0) {
-    {
+    } else if (warp == 0) {
       // ===== weight (B) producer: one [BN][64] tile per plane per (channel block, tap) =====
       int s = 0;
       uint32_t ph = 0;
@@ -215,87 +189,106 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    {
-      // ===== MMA issuer (whole warp runs the loop; one elected lane issues) =====
-      // Descriptors are (per-stage low word) + compile-time offsets: planes, taps and k-slices are fully
-      // unrolled so every tcgen05.mma needs only two uniform adds (N = 64 tiles are issue-rate bound).
-      constexpr uint32_t kPatch16 = (TAPS == 9 ? 23552u : 16384u) >> 4;   // plane stride of the A stage, in 16-B units
-      constexpr uint32_t kB16 = (uint32_t)kBBytes >> 4;
-      constexpr uint32_t kHiB = (1024u >> 4) | (1u << 14) | (2u << 29);    // SBO | version | SWIZZLE_128B
-      const uint32_t hi_a = ((uint32_t)p.group_stride_bytes >> 4) | (1u << 14) | (2u << 29);
-      int sa = 0, sb = 0, a = 0;
-      uint32_t pha = 0, phb = 0, aph = 0;
-      for (int u = u_begin; u < p.total_units; u += u_step) {
-        mbar_wait(tempty0 + 8 * a, aph ^ 1u);
-        tc_fence_after();
-        const uint32_t d_main = tmem_base + (uint32_t)a * acc_cols, d_cross = d_main + BN;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(fullA + 8 * sa, pha);
-          const uint32_t a_lo = (((ring_a + sa * a_stage) >> 4) & 0x3FFFu) | (1u << 16);
+  } else {
+    regs_alloc<232>();
+    // ===== consumers: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64) (pixel tile rows 8 wg .. 8 wg + 7) against all
+    // BN channels, then both warpgroups run the epilogue of the tile through a float32 staging buffer =====
+    const int wg = (warp >> 2) - 1;
+    const bool leader = (threadIdx.x & 127) == 0;
+    constexpr int R = BN / 2;                  // accumulator registers per thread (64 x BN per warpgroup)
+    float accm[R], accc[R];                    // main and (P > 1) cross accumulators
+    // Descriptors are (per-stage low word) + compile-time offsets: planes, taps and k-slices are fully unrolled.
+    constexpr uint32_t kPatch16 = (TAPS == 9 ? 23552u : 16384u) >> 4;   // plane stride of the A stage, in 16-B units
+    constexpr uint32_t kB16 = (uint32_t)kBBytes >> 4;
+    constexpr uint32_t kHiB = gmma_desc_hi(1024);
+    const uint32_t hi_a = gmma_desc_hi((uint32_t)p.group_stride_bytes);
+    const uint32_t wg_off = (uint32_t)wg * 8u * (uint32_t)p.group_stride_bytes;   // 8 row groups of 8 pixels per warpgroup
+    // epilogue geometry: consumer warp cw = set (even / odd 32-channel chunks) x quarter of the 128 pixels; thread = pixel m
+    const int cw = warp - 4, eset = cw >> 2, quarter = cw & 3;
+    const int m = quarter * 32 + lane;
+    const int th = m >> p.tw_log2, tw = m & (p.TW - 1);
+    const bool pool = (p.flags & CTPN_F_POOL) != 0, relu = (p.flags & CTPN_F_RELU) != 0;
+    const bool out_f32 = (p.flags & CTPN_F_OUT_F32) != 0;
+    int sa = 0, sb = 0, prev_b = -1, prev_a = -1;
+    uint32_t pha = 0, phb = 0;
+    // a weight stage (and after its last tap an activation stage) is released once the MMAs that read it have completed
+    auto release = [&](int sbx, int sax) {
+      if (leader) {
+        if (MC) {
+          mbar_arrive_cluster(emptyB + 8 * sbx, 0u);
+          mbar_arrive_cluster(emptyB + 8 * sbx, 1u);
+        } else {
+          mbar_arrive(emptyB + 8 * sbx);
+        }
+        if (sax >= 0) mbar_arrive(emptyA + 8 * sax);
+      }
+    };
+    for (int u = u_begin; u < p.total_units; u += u_step) {
+      for (int kb = 0; kb < kblocks; ++kb) {
+        if (p.stages_a == 1 && prev_a >= 0) {   // a single activation stage: it must be free before its next load
+          wgmma_wait<0>();
+          release(prev_b, prev_a);
+          prev_b = prev_a = -1;
+        }
+        mbar_wait(fullA + 8 * sa, pha);
+        const uint32_t a_lo = gmma_desc_lo(ring_a + sa * a_stage + wg_off);
 #pragma unroll
-          for (int tap = 0; tap < TAPS; ++tap) {
-            mbar_wait(fullB + 8 * sb, phb);
-            tc_fence_after();
-            const uint32_t b_lo = (((ring_b + sb * b_stage) >> 4) & 0x3FFFu) | (1u << 16);
-            constexpr int kPW = 10;
-            const uint32_t view16 = TAPS == 9 ? (uint32_t)((tap / 3) * kPW + tap % 3) * 8u : 0u;
-            const uint32_t not_first = (kb | tap) != 0;
+        for (int tap = 0; tap < TAPS; ++tap) {
+          mbar_wait(fullB + 8 * sb, phb);
+          const uint32_t b_lo = gmma_desc_lo(ring_b + sb * b_stage);
+          constexpr int kPW = 10;
+          const uint32_t view16 = TAPS == 9 ? (uint32_t)((tap / 3) * kPW + tap % 3) * 8u : 0u;
+          const uint32_t not_first = (kb | tap) != 0;
+          wgmma_fence();
+          if (!CTPN_DBG(p, 4)) {
             if (F8) {
-              if (elect_one() && !CTPN_DBG(p, 4)) {
 #pragma unroll
-                for (int k = 0; k < 4; ++k)     // fp16 x fp16, K = 16 (32 B) per instruction
-                  mma_bf16_ss(d_main, ((uint64_t)hi_a << 32) | (a_lo + view16 + 2u * k), ((uint64_t)kHiB << 32) | (b_lo + 2u * k), kIdesc,
-                              k == 0 ? not_first : 1u);
+              for (int k = 0; k < 4; ++k)     // fp16 x fp16, K = 16 (32 B) per instruction
+                wgmma_f16(accm, ((uint64_t)hi_a << 32) | (a_lo + view16 + 2u * k), ((uint64_t)kHiB << 32) | (b_lo + 2u * k),
+                          k == 0 ? not_first : 1u);
 #pragma unroll
-                for (int k = 0; k < 4; ++k)     // e4m3 x e4m3, K = 32 (32 B): k 0,1 = value x residual, k 2,3 = residual x value
-                  mma_f8_ss(d_cross, ((uint64_t)hi_a << 32) | (a_lo + kPatch16 + view16 + 2u * k),
-                            ((uint64_t)kHiB << 32) | (b_lo + kB16 + 2u * k), kIdesc8, k == 0 ? not_first : 1u);
-              }
-            } else if (elect_one() && !CTPN_DBG(p, 4)) {
+              for (int k = 0; k < 4; ++k)     // e4m3 x e4m3, K = 32 (32 B): k 0,1 = value x residual, k 2,3 = residual x value
+                wgmma_e4m3(accc, ((uint64_t)hi_a << 32) | (a_lo + kPatch16 + view16 + 2u * k),
+                           ((uint64_t)kHiB << 32) | (b_lo + kB16 + 2u * k), k == 0 ? not_first : 1u);
+            } else {
 #pragma unroll
               for (int i = 0; i < P; ++i) {
 #pragma unroll
                 for (int j = 0; j < P - i; ++j) {
 #pragma unroll
-                  for (int k = 0; k < 4; ++k) {   // 64 / UMMA_K(16); +32 B == +2 in the >>4 address field
+                  for (int k = 0; k < 4; ++k) {   // 64 / K(16); +32 B == +2 in the >>4 address field
                     const uint64_t da = ((uint64_t)hi_a << 32) | (a_lo + i * kPatch16 + view16 + 2u * k);
                     const uint64_t db = ((uint64_t)kHiB << 32) | (b_lo + j * kB16 + 2u * k);
-                    if (i + j == 0) mma_bf16_ss(d_main, da, db, kIdesc, k == 0 ? not_first : 1u);
-                    else mma_bf16_ss(d_cross, da, db, kIdesc, (k == 0 && i == 0 && j == 1) ? not_first : 1u);
+                    if (i + j == 0) wgmma_bf16(accm, da, db, k == 0 ? not_first : 1u);
+                    else wgmma_bf16(accc, da, db, (k == 0 && i == 0 && j == 1) ? not_first : 1u);
                   }
                 }
               }
             }
-            __syncwarp();
-            if (elect_one()) {                              // weight stage free once these MMAs have read it
-              if (MC) mma_commit_mc(emptyB + 8 * sb, (uint16_t)3);   // ... in both CTAs: the peer multicasts into it too
-              else mma_commit(emptyB + 8 * sb);
-            }
-            __syncwarp();
-            if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
           }
-          if (elect_one()) mma_commit(emptyA + 8 * sa);     // halo patch free after its last tap
-          __syncwarp();
-          if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
+          wgmma_commit();
+          wgmma_wait<1>();                   // the previous step's MMAs are done: free its stages
+          if (prev_b >= 0) release(prev_b, prev_a);
+          prev_b = sb;
+          prev_a = tap == TAPS - 1 ? sa : -1;
+          if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
         }
-        if (elect_one()) mma_commit(tfull0 + 8 * a);        // accumulator complete -> epilogue
-        __syncwarp();
-        if (++a == p.nbuf) { a = 0; aph ^= 1u; }
+        if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
       }
-    }
-  } else if (warp != 6) {
-    // ===== epilogue: two sets of four warps (TMEM lane quarter = warp id % 4); set 0 takes the even 32-column
-    // chunks of the accumulator, set 1 the odd ones =====
-    const int quarter = warp & 3;
-    const int eset = warp >= 7 ? 1 : 0, ewarp = warp >= 7 ? warp - 3 : warp - 2;
-    const int m = quarter * 32 + lane;
-    const int th = m >> p.tw_log2, tw = m & (p.TW - 1);
-    const bool pool = (p.flags & CTPN_F_POOL) != 0, relu = (p.flags & CTPN_F_RELU) != 0;
-    const bool out_f32 = (p.flags & CTPN_F_OUT_F32) != 0;
-    int a = 0;
-    uint32_t aph = 0;
-    for (int u = u_begin; u < p.total_units; u += u_step) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(accm);
+      if (P > 1) wgmma_fence_regs(accc);
+      if (prev_b >= 0) release(prev_b, prev_a);
+      prev_b = prev_a = -1;
+      // main (+ cross): kept apart during the K loop because the tensor core truncates when it adds into float32
+      if (P > 1) {
+#pragma unroll
+        for (int i = 0; i < R; ++i) accm[i] = F8 ? __fmaf_rn(accc[i], p.inv_cross, accm[i] * p.inv_main) : accm[i] + accc[i];
+      }
+
+      // ===== epilogue: +bias -> ReLU -> optional fused 2x2 max-pool (warp shuffles: the window of a pixel lives in lanes
+      // l, l^1, l^8, l^9) -> re-split into planes -> transpose through swizzled shared memory -> 16-byte stores that cover
+      // one pixel's 64 contiguous bytes with 4 lanes (or float32 output) =====
       int mt, nt;
       unit_tile(u, mt, nt);
       const int b = mt / tiles_per_img, r = mt % tiles_per_img;
@@ -327,31 +320,32 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         const unsigned lo = __shfl_sync(0xffffffffu, (unsigned)(pix & 0xffffffffll), it * 8 + (lane >> 2));
         spix[it] = (hi << 32) | lo;
       }
-      uint4 *stage_w = reinterpret_cast<uint4 *>(stage_buf + ewarp * (p.stage_small ? 8 : 32) * kStagePitch);
-      mbar_wait(tfull0 + 8 * a, aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)a * acc_cols;
-#pragma unroll 1
-      for (int chunk = eset; chunk < (CTPN_DBG(p, 16) ? 0 : BN / 32); chunk += 2) {
-        uint32_t rr[32];
-        tmem_ld_32x32(taddr + chunk * 32, rr);
+      // float32 staging [2 chunks][128 pixels][32 channels], 16-byte chunks XOR-swizzled by pixel & 7; the 32 rows a warp
+      // reads back are its own, and once read they serve as its store-transpose block
+      uint4 *stage_w = reinterpret_cast<uint4 *>(epi + eset * 4096 + quarter * 1024);
+      const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // accumulator fragment rows frow, frow + 8
+      if (!CTPN_DBG(p, 16)) {
+#pragma unroll
+      for (int c2 = 0; c2 < BN / 64; ++c2) {
+        named_sync(1, 256);           // the previous chunk pair has been read
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int i8 = c2 * 8 + j, q = 2 * (j & 3) + ((lane & 3) >> 1);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = frow + 8 * h;
+            *reinterpret_cast<float2 *>(epi + (j >> 2) * 4096 + row * 32 + ((q ^ (row & 7)) << 2) + 2 * (lane & 1)) =
+                make_float2(accm[4 * i8 + 2 * h], accm[4 * i8 + 2 * h + 1]);
+          }
+        }
+        named_sync(1, 256);
+        const int chunk = 2 * c2 + eset;
         const int c0 = nt * BN + chunk * 32;
         float v[32];
-        if (P > 1) {
-          uint32_t rc[32];
-          tmem_ld_32x32(taddr + BN + chunk * 32, rc);     // both accumulators in flight, one wait
-          tmem_ld_wait();
-          if (F8) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __fmaf_rn(__uint_as_float(rc[i]), p.inv_cross, __uint_as_float(rr[i]) * p.inv_main);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]) + __uint_as_float(rc[i]);
-          }
-        } else {
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rr[i]);
+        for (int q = 0; q < 8; ++q) {
+          const float4 t = *reinterpret_cast<const float4 *>(epi + eset * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
+          v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
         }
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
@@ -484,20 +478,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * a);
-      if (++a == p.nbuf) { a = 0; aph ^= 1u; }
+      }
     }
   }
-  tc_fence_before();
   __syncthreads();
   if (MC) cluster_sync_all();      // no CTA leaves while its peer can still signal its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.nbuf * acc_cols);
-  }
 }
+
 
 // ---- host side -------------------------------------------------------------------------------
 // Per-device launch state: SM count, the dynamic-shared-memory attribute and the co-resident cluster count of every
@@ -566,23 +553,22 @@ static int cached_tmap(int dev, CUtensorMap *out, const void *ptr, int rank, con
 template <int BN, int P, int TAPS, int MC, int F8 = 0>
 static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, ConvTcParams &p, cudaStream_t st) {
   const size_t a_stage = (size_t)p.planes * p.patch_bytes, b_stage = (size_t)p.planes * BN * 128;
-  // long-K F16F8 layers: a quarter-size staging block buys a 4th weight stage (their weight stream, not the epilogue, is
-  // what the tensor pipe waits for: 3 stages x 280 ns of MMAs do not cover the L2 latency)
+  // long-K F16F8 layers store through 8-pixel rounds (a 512-byte transpose block per warp)
   const bool small = F8 && TAPS == 9 && p.Cin >= 256 && !(p.flags & (CTPN_F_OUT_F32 | CTPN_F_OUT_BF16X2 | CTPN_F_POOL)) && tuning().stage_small != 0;
   p.stage_small = small ? 1 : 0;
-  const size_t stage_bytes = small ? kStageBytes / 4 : kStageBytes;
-  const size_t budget = 227 * 1024 - 1024 - kCtrlBytes - stage_bytes;
+  const size_t budget = 227 * 1024 - 1024 - kCtrlBytes - kEpiBytes;
   // activation ring: two stages when they leave room for at least two weight stages, else one
   int sa = (2 * a_stage + 2 * b_stage <= budget) ? 2 : 1;
   if (p.taps == 1) sa = (int)std::min<size_t>(4, std::max<size_t>(1, (budget / 2) / a_stage));
-  CTPN_REQUIRE(sa * a_stage + b_stage <= budget, "conv_tc: pipeline stages (%zu + %zu B) do not fit in shared memory", a_stage, b_stage);
+  // at least two weight stages: the consumers free a stage only after the MMAs of the following one have been issued
+  CTPN_REQUIRE(sa * a_stage + 2 * b_stage <= budget, "conv_tc: pipeline stages (%zu + 2 x %zu B) do not fit in shared memory", a_stage, b_stage);
   int sb = (int)((budget - sa * a_stage) / b_stage);
   if (sb > kMaxStages) sb = kMaxStages;
   if (tuning().stages_a > 0) sa = std::max(1, std::min(sa, tuning().stages_a));
-  if (tuning().stages_b > 0) sb = std::max(1, std::min(sb, tuning().stages_b));
+  if (tuning().stages_b > 0) sb = std::max(2, std::min(sb, tuning().stages_b));
   p.stages_a = sa;
   p.stages_b = sb;
-  const size_t smem = 1024 + sa * a_stage + sb * b_stage + stage_bytes + kCtrlBytes;
+  const size_t smem = 1024 + sa * a_stage + sb * b_stage + kEpiBytes + kCtrlBytes;
   CTPN_REQUIRE(smem <= 227 * 1024, "conv_tc: %zu bytes of shared memory", smem);
   auto kernel = conv_tc_kernel<BN, P, TAPS, MC, F8>;
   static bool attr_set[kMaxDevices];
@@ -658,7 +644,7 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   ConvTcParams p;
   memset(&p, 0, sizeof(p));
   p.B = B; p.H = H; p.W = W; p.Cin = cin; p.Cout = cout; p.taps = taps; p.planes = planes; p.flags = flags;
-  if (taps == 9) {   // 16 x 8 pixel tile: one 8-row UMMA group per tile row, halo patch 18 x 10
+  if (taps == 9) {   // 16 x 8 pixel tile: one 8-row wgmma group per tile row, halo patch 18 x 10
     p.TH = 16; p.TW = 8; p.tw_log2 = 3;
     p.PW = 10;
     p.group_stride_bytes = p.PW * 128;
@@ -691,14 +677,13 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   }
   p.debug = tuning().debug;
 
-  // N tile: 256 halves the A traffic per MAC but, with two accumulators per tile (P > 1), leaves no TMEM for
-  // double buffering -- worth it only when the K loop is long enough to amortise the serialised epilogue.
+  // N tile: 256 halves the A traffic per MAC; with two accumulators per tile (P > 1) it would need 256 accumulator
+  // registers per consumer thread, so those stay at 128.
   int BN = tuning().bn > 0 ? tuning().bn : (planes == 1 ? 256 : 128);
   if (!(BN == 64 || BN == 128 || BN == 256)) BN = 256;
-  if (planes > 1 && BN > 128) BN = 128;   // main + cross accumulators, double buffered: 4 * BN TMEM columns <= 512 (F16F8 too)
+  if (planes > 1 && BN > 128) BN = 128;   // main + cross accumulators: 2 * BN / 2 registers per thread (F16F8 too)
   while (BN > cout || cout % BN) BN >>= 1;
   p.tiles_n = cout / BN;
-  p.nbuf = ((planes > 1 ? 2 : 1) * BN * 2 <= 512) ? 2 : 1;   // 512 TMEM columns per SM
   const long long m_tiles = (long long)B * p.tiles_x * p.tiles_y;
   const long long total = m_tiles * p.tiles_n;
   CTPN_REQUIRE(total < (1ll << 31), "ctpn_conv3x3: too many tiles");
@@ -738,13 +723,13 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
     return CTPN_ERR_INVALID;
   }
   CTPN_TC_CASE_MC(256, 1); CTPN_TC_CASE_MC(128, 1); CTPN_TC_CASE_MC(64, 1);
-  CTPN_TC_CASE_MC(256, 2); CTPN_TC_CASE_MC(128, 2); CTPN_TC_CASE_MC(64, 2);
+  CTPN_TC_CASE_MC(128, 2); CTPN_TC_CASE_MC(64, 2);
   CTPN_TC_CASE_MC(128, 3); CTPN_TC_CASE_MC(64, 3);
   CTPN_TC_CASE(256, 1, 9); CTPN_TC_CASE(128, 1, 9); CTPN_TC_CASE(64, 1, 9);
-  CTPN_TC_CASE(256, 2, 9); CTPN_TC_CASE(128, 2, 9); CTPN_TC_CASE(64, 2, 9);
+  CTPN_TC_CASE(128, 2, 9); CTPN_TC_CASE(64, 2, 9);
   CTPN_TC_CASE(128, 3, 9); CTPN_TC_CASE(64, 3, 9);
   CTPN_TC_CASE(256, 1, 1); CTPN_TC_CASE(128, 1, 1); CTPN_TC_CASE(64, 1, 1);
-  CTPN_TC_CASE(256, 2, 1); CTPN_TC_CASE(128, 2, 1); CTPN_TC_CASE(64, 2, 1);
+  CTPN_TC_CASE(128, 2, 1); CTPN_TC_CASE(64, 2, 1);
   CTPN_TC_CASE(128, 3, 1); CTPN_TC_CASE(64, 3, 1);
 #undef CTPN_TC_CASE_MC
 #undef CTPN_TC_CASE

@@ -23,6 +23,19 @@ int cuda_fail(cudaError_t e, const char *what, const char *file, int line) {
   set_error("CUDA error %d (%s) at %s:%d: %s", (int)e, cudaGetErrorString(e), file, line, what);
   return e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver ? CTPN_ERR_NO_DEVICE : CTPN_ERR_CUDA;
 }
+
+int current_sm_count(int *sms) {
+  constexpr int kMaxDevices = 64;
+  static std::mutex mu;
+  static int cache[kMaxDevices];
+  int dev = 0;
+  CTPN_CUDA(cudaGetDevice(&dev));
+  CTPN_REQUIRE(dev >= 0 && dev < kMaxDevices, "device index %d not supported", dev);
+  std::lock_guard<std::mutex> lock(mu);
+  if (cache[dev] == 0) CTPN_CUDA(cudaDeviceGetAttribute(&cache[dev], cudaDevAttrMultiProcessorCount, dev));
+  *sms = cache[dev];
+  return CTPN_OK;
+}
 }  // namespace ctpn
 
 // ---- optional per-launch timing (CUDA events on the launching stream) --------------------------
@@ -104,8 +117,8 @@ extern "C" int ctpn_device_ok(int device_id) {
   }
   int major = 0;
   CTPN_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device_id));
-  if (major != 10) {
-    ctpn::set_error("device %d has compute capability %d.x; this library is sm_100a only", device_id, major);
+  if (major != 9) {
+    ctpn::set_error("device %d has compute capability %d.x; this library is sm_90a only", device_id, major);
     return CTPN_ERR_NO_DEVICE;
   }
   return CTPN_OK;

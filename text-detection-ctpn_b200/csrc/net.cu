@@ -1,6 +1,6 @@
 // ctpn_net_*: the CTPN test graph up to the two head tensors, as one stream-ordered sequence of
 // the stage kernels (lib/networks/VGGnet_test.py:16-52; variable names per SURVEY.md App. A.2).
-//   uint8 image -> conv1_1 (tcgen05, fused mean subtraction) -> 13 x tcgen05 conv (+fused pools)
+//   uint8 image -> conv1_1 (wgmma, fused mean subtraction) -> 13 x wgmma conv (+fused pools)
 //   -> x-projection GEMM -> BiLSTM recurrence (2-CTA clusters) -> FC GEMM -> heads GEMM.
 // Weights live in library-owned device memory; activations in the caller's workspace.
 #include <algorithm>

@@ -150,7 +150,10 @@ int nms_sorted_launch(const float *boxes, const int *counts, int batch, int max_
   CTPN_REQUIRE(((uintptr_t)boxes & 15) == 0, "ctpn_nms_sorted: boxes must be 16-byte aligned");
   u64 *mask = reinterpret_cast<u64 *>(workspace);
   long long pairs = (long long)cb * cb;
-  const unsigned grid = (unsigned)(pairs < 148 * 16 ? pairs : 148 * 16);
+  int sms = 0;
+  if (int rc = current_sm_count(&sms)) return rc;
+  const long long cap = 16ll * sms;        // grid-stride loop: 16 CTAs per SM
+  const unsigned grid = (unsigned)(pairs < cap ? pairs : cap);
   ProfScope prof("nms (mask+scan)", 0.0, st);
   nms_mask_kernel<<<grid, kNmsTile, 0, st>>>(reinterpret_cast<const float4 *>(boxes), counts, batch, max_n, cb, thresh, mask, gate);
   CTPN_LAUNCH_CHECK();

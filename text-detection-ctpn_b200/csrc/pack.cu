@@ -1,5 +1,5 @@
 // Weight packing for the tensor-core layers: TF-layout float32 weights [taps][Cin][Cout] (HWIO flattened,
-// lib/networks/network.py:160-170) -> bf16 planes [P][Cout_pad][taps][Cin] (K-major rows of the UMMA B operand).
+// lib/networks/network.py:160-170) -> bf16 planes [P][Cout_pad][taps][Cin] (K-major rows of the wgmma B operand).
 #include "common.cuh"
 
 namespace ctpn {

@@ -145,7 +145,9 @@ extern "C" int ctpn_resize_linear_u8(const void *src, int B, int sh, int sw, int
   const double scale_x = 1.0 / fx, scale_y = 1.0 / fy;
   const int area2 = (scale_x == 2.0 && scale_y == 2.0) ? 1 : 0;   // cv::resize routes exact 2x decimation to INTER_AREA
   const long long total = (long long)B * dh * dw;
-  const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 32);
+  int sms = 0;
+  if ((rc = current_sm_count(&sms))) return rc;
+  const int grid = (int)std::min<long long>((total + 255) / 256, 32LL * sms);   // grid-stride loop: 32 CTAs per SM
   ProfScope prof("resize_linear_u8", (double)total * channels, (cudaStream_t)stream);
   resize_linear_u8_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src, (uint8_t *)dst, B, sh, sw, channels,
                                                                   dh, dw, scale_x, scale_y, area2);
@@ -164,7 +166,9 @@ extern "C" int ctpn_image_blob_f32(const void *src_u8, const float *lut, int B, 
   const double scale_x = 1.0 / fx, scale_y = 1.0 / fy;
   const int area2 = (scale_x == 2.0 && scale_y == 2.0) ? 1 : 0;
   const long long total = (long long)B * dh * dw;
-  const int grid = (int)std::min<long long>((total + 255) / 256, 148LL * 32);
+  int sms = 0;
+  if ((rc = current_sm_count(&sms))) return rc;
+  const int grid = (int)std::min<long long>((total + 255) / 256, 32LL * sms);   // grid-stride loop: 32 CTAs per SM
   ProfScope prof("image_blob_f32", (double)total * 3, (cudaStream_t)stream);
   image_blob_f32_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src_u8, lut, dst, B, sh, sw, dh, dw, scale_x,
                                                                 scale_y, area2);

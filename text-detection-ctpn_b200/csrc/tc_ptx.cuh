@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by conv_tc.cu:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA, TMEM alloc/ld, commit, fences).
+// Thin inline-PTX wrappers for the Hopper (sm_90a) async machinery used by conv_tc.cu and conv1_tc.cu:
+// mbarrier, TMA (cp.async.bulk.tensor), thread-block clusters and wgmma (warpgroup MMA from shared-memory descriptors).
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -48,15 +48,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.  No printf here: a
+// function call anywhere in a kernel that issues wgmma makes the compiler serialise its MMAs.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {   // ~2 s at 2 GHz
-      printf("ctpn: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s at 2 GHz
   }
 }
 
@@ -96,85 +94,79 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   return r;
 }
 
-// ---- tcgen05 -------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (this CTA included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(bar), "r"(cta) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 x bf16 -> f32, M=128 (cta_group::1)
-__device__ __forceinline__ void mma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+// named barrier over `count` threads (whole warps)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-// D[tmem] (+)= A * B with 8-bit float operands (kind::f8f6f4; formats from the instruction descriptor), K = 32, M=128
-__device__ __forceinline__ void mma_f8_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void mma_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(cta_mask) : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread = TMEM lane)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
+// ---- warpgroup register budget -----------------------------------------------------------------
+template <uint32_t R> __device__ __forceinline__ void regs_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void regs_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// ---- wgmma ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator registers across the asynchronous MMAs that own them
+template <int R> __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// K-major SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA):
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1)
-//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024) | [46,48) version = 1 | [61,64) layout = 2
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// cute::UMMA::InstrDescriptor for kind::f16: D=f32 (bit 4), A=B=bf16 (bits 7,10), K-major A and B,
-// N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+//   [32,46) stride byte offset >> 4 (between 8-row groups) | [49,52) base offset 0 | [62,64) layout 1 = SWIZZLE_128B
+// The swizzle is a function of the absolute shared-memory address (the same one TMA applies when it writes a
+// 1024-aligned box), so views that start at any 128-byte row of a swizzled buffer read it consistently.
+__host__ __device__ constexpr uint32_t gmma_desc_hi(uint32_t stride_bytes) { return (stride_bytes >> 4) | (1u << 30); }
+__device__ __forceinline__ uint32_t gmma_desc_lo(uint32_t smem_addr) { return ((smem_addr >> 4) & 0x3FFFu) | (1u << 16); }
 
-// kind::f16 with fp16 (format code 0) operands; kind::f8f6f4 with e4m3 (format code 0) operands; D = f32
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t umma_idesc_e4m3(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in shared memory, f32 accumulators in registers (fragment
+// layout: d[4 i + 2 h + e] = row 16 (warp % 4) + lane / 4 + 8 h, column 8 i + 2 (lane % 4) + e); acc = 0 overwrites D.
+// bf16 / fp16: K = 16 (32 bytes) per instruction; e4m3: K = 32 (32 bytes).
+#define CTPN_WGMMA_N64(NAME, KTYPE, TRANS)                                                                   \
+  __device__ __forceinline__ void NAME(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {              \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                          \
+                 "wgmma.mma_async.sync.aligned.m64n64" KTYPE " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1" TRANS ";\n\t}" \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+                 : "l"(da), "l"(db), "r"(acc));                                                      \
+  }
+#define CTPN_WGMMA_N128(NAME, KTYPE, TRANS)                                                                   \
+  __device__ __forceinline__ void NAME(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {              \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                          \
+                 "wgmma.mma_async.sync.aligned.m64n128" KTYPE " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1" TRANS ";\n\t}" \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+                 : "l"(da), "l"(db), "r"(acc));                                                      \
+  }
+#define CTPN_WGMMA_N256(NAME, KTYPE, TRANS)                                                                   \
+  __device__ __forceinline__ void NAME(float (&d)[128], uint64_t da, uint64_t db, uint32_t acc) {              \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                          \
+                 "wgmma.mma_async.sync.aligned.m64n256" KTYPE " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1" TRANS ";\n\t}" \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127]) \
+                 : "l"(da), "l"(db), "r"(acc));                                                      \
+  }
+
+CTPN_WGMMA_N64(wgmma_bf16, "k16.f32.bf16.bf16", ", 0, 0")
+CTPN_WGMMA_N128(wgmma_bf16, "k16.f32.bf16.bf16", ", 0, 0")
+CTPN_WGMMA_N256(wgmma_bf16, "k16.f32.bf16.bf16", ", 0, 0")
+CTPN_WGMMA_N64(wgmma_f16, "k16.f32.f16.f16", ", 0, 0")
+CTPN_WGMMA_N128(wgmma_f16, "k16.f32.f16.f16", ", 0, 0")
+CTPN_WGMMA_N256(wgmma_f16, "k16.f32.f16.f16", ", 0, 0")
+CTPN_WGMMA_N64(wgmma_e4m3, "k32.f32.e4m3.e4m3", "")
+CTPN_WGMMA_N128(wgmma_e4m3, "k32.f32.e4m3.e4m3", "")
+CTPN_WGMMA_N256(wgmma_e4m3, "k32.f32.e4m3.e4m3", "")
+#undef CTPN_WGMMA_N64
+#undef CTPN_WGMMA_N128
+#undef CTPN_WGMMA_N256
 
 }  // namespace ptx
 }  // namespace ctpn

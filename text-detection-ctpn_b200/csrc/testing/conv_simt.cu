@@ -2,7 +2,7 @@
 //   * ctpn_conv1_1        first VGG layer (Cin = 3, K = 27: HBM-bound, no tensor cores); fuses the
 //                         uint8 -> float32 mean subtraction of lib/fast_rcnn/test.py:8-9
 //   * ctpn_conv3x3_simt   same contract as ctpn_conv3x3 with plain float32 FMAs: the in-library
-//                         reference the tests use to validate the tcgen05 kernel
+//                         reference the tests use to validate the wgmma kernel
 // Reference semantics: lib/networks/network.py:160-196.
 #include "../common.cuh"
 #include "ctpn_b200_testing.h"

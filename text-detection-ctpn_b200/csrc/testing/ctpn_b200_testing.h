@@ -1,6 +1,6 @@
 /*
  * Test-only entry points of libctpn_b200_dbg.so (tests/_native/): float32 SIMT reference kernels with the product
- * kernels' contracts, and hardware probes.  None of this is in the product library libctpn_b200.so or in
+ * kernels' contracts, and a hardware probe.  None of this is in the product library libctpn_b200.so or in
  * include/ctpn_b200.h.  The debug library is the product sources compiled with -DCTPN_DEBUG (ablation switches
  * CTPN_TC_DEBUG / CTPN_C1_DEBUG, tuning overrides CTPN_TC_BN / CTPN_TC_STAGES_* / CTPN_TC_MCAST, the "conv_simt" /
  * "conv1_simt" options of ctpn_net_set_option) plus the two files in this directory.
@@ -29,24 +29,11 @@ int ctpn_conv3x3_simt(const void *in_planes, const void *w_planes, const float *
 
 
 /* ---- hardware probes ---------------------------------------------------------------------
- * Hardware probe used by tests/probe_umma_view.py: reads a [rows][64] bf16 matrix through a UMMA
+ * Hardware probe used by tests/probe_umma_view.py: reads a [rows][64] bf16 matrix through a wgmma
  * K-major SWIZZLE_128B descriptor that starts at row `row0` with `group_stride_rows` between 8-row
  * groups, against the identity, and returns the 128x64 values the tensor core fetched. */
 int ctpn_probe_umma_view(const void *a_bf16, const void *identity_bf16, int rows, int row0,
                          int group_stride_rows, int base_offset_mode, float *out, void *stream);
-
-/* Hardware probe: every CTA issues n_mma 128 x bn x 16 bf16 MMAs with a tcgen05.commit every
- * `commit_every` MMAs and (lag > 0) waits on each commit `lag` commits later.  Timed by the caller. */
-int ctpn_probe_mma_rate(int bn, int n_mma, int commit_every, int lag, int alternate_acc, int fence_each,
-                        int grid, void *stream);
-
-/* Hardware probe: the same back-to-back issue loop with cta_group::2 instructions (M = 256 over a 2-CTA cluster,
- * each CTA holding its 128 A rows and bn/2 rows of B).  grid must be even; n_mma a multiple of 8. */
-int ctpn_probe_mma_rate_pair(int bn, int n_mma, int alternate_acc, int grid, void *stream);
-
-/* Hardware probe: dispatch rate of kind::f8f6f4 (e4m3, K = 32) next to kind::f16 (K = 16) from one CTA (pair = 0, M = 128)
- * or a CTA pair (pair = 1, cta_group::2, M = 256).  mode 0 all f16, 1 all f8, 2 groups of 4 f16 + 4 f8 on two accumulators. */
-int ctpn_probe_mma_kind(int bn, int pair, int mode, int n_mma, int grid, void *stream);
 
 #ifdef __cplusplus
 }

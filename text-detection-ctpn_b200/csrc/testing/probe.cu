@@ -1,11 +1,11 @@
-// Diagnostic probe (not on the product path): which shared-memory rows does a K-major SWIZZLE_128B UMMA
+// Diagnostic probe (not on the product path): which shared-memory rows does a K-major SWIZZLE_128B wgmma
 // A-descriptor fetch when its start address is NOT 1024-byte aligned and its 8-row groups are spaced by an
 // arbitrary stride?  The answer decides whether the 9 taps of a 3x3 convolution can be served as shifted
 // VIEWS of one halo patch in shared memory instead of 9 separate TMA loads.
 //
 // A [rows][64] bf16 matrix is TMA-loaded (128B swizzle) into 1024-aligned shared memory; B is the 64x64
 // identity, so D[m][n] = A_view[m][n]: the output reveals, for every (m, 16-byte chunk), the element the
-// tensor core actually read.
+// tensor core actually read.  One warpgroup, two m64n64k16 passes (view rows 0-63 and 64-127).
 #include <cuda.h>
 
 #include "../common.cuh"
@@ -23,51 +23,37 @@ probe_umma_view_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t sa = (raw + 1023u) & ~1023u;          // A: rows x 128 B
   const uint32_t sb = sa + ((rows * 128 + 1023) & ~1023);   // B: 64 x 128 B
-  __shared__ uint64_t bars[2];
-  __shared__ uint32_t tmem_slot;
-  const uint32_t bar_load = smem_u32(&bars[0]), bar_mma = smem_u32(&bars[1]);
+  __shared__ uint64_t bar;
+  const uint32_t bar_load = smem_u32(&bar);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(bar_load, 1);
-    mbar_init(bar_mma, 1);
     fence_mbar_init();
   }
-  if (warp == 0) { tmem_alloc(smem_u32(&tmem_slot), 64); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(bar_load, (uint32_t)(rows * 128 + 64 * 128));
     for (int r = 0; r < rows; r += 64) tma_load_2d(&tmap_a, bar_load, sa + r * 128, 0, r);   // box = 64 x 64
     tma_load_2d(&tmap_b, bar_load, sb, 0, 0);
-    mbar_wait(bar_load, 0);
-    tc_fence_after();
-    const uint32_t start = sa + (uint32_t)row0 * 128u;
-    uint64_t da = 0;
-    da |= (uint64_t)((start >> 4) & 0x3FFF);
-    da |= (uint64_t)1 << 16;
-    da |= (uint64_t)(((uint32_t)group_stride_rows * 128u) >> 4) << 32;
-    da |= (uint64_t)1 << 46;
-    if (base_offset_mode == 1) da |= (uint64_t)((start >> 7) & 7u) << 49;
-    da |= (uint64_t)2 << 61;
-    const uint64_t db = umma_desc_k_sw128(sb);
-    const uint32_t idesc = umma_idesc_bf16(128, 64);
-    for (int k = 0; k < 4; ++k) mma_bf16_ss(tmem, da + 2ull * k, db + 2ull * k, idesc, k > 0);
-    mma_commit(bar_mma);
   }
-  __syncthreads();
-  mbar_wait(bar_mma, 0);
-  tc_fence_after();
-  for (int chunk = 0; chunk < 2; ++chunk) {
-    uint32_t rr[32];
-    tmem_ld_32x32(tmem + ((uint32_t)(warp * 32) << 16) + chunk * 32, rr);
-    tmem_ld_wait();
-    for (int i = 0; i < 32; ++i) out[(warp * 32 + lane) * 64 + chunk * 32 + i] = __uint_as_float(rr[i]);
+  mbar_wait(bar_load, 0);
+  const uint64_t db = ((uint64_t)gmma_desc_hi(1024) << 32) | gmma_desc_lo(sb);
+  for (int half = 0; half < 2; ++half) {
+    const uint32_t start = sa + (uint32_t)(row0 + half * 8 * group_stride_rows) * 128u;
+    uint32_t hi = gmma_desc_hi((uint32_t)group_stride_rows * 128u);
+    if (base_offset_mode == 1) hi |= ((start >> 7) & 7u) << 17;     // descriptor bits [49,52)
+    const uint64_t da = ((uint64_t)hi << 32) | gmma_desc_lo(start);
+    float d[32];
+    wgmma_fence();
+    for (int k = 0; k < 4; ++k) wgmma_bf16(d, da + 2ull * k, db + 2ull * k, k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(d);
+    for (int i = 0; i < 8; ++i)
+      for (int h = 0; h < 2; ++h)
+        for (int e = 0; e < 2; ++e)
+          out[(half * 64 + warp * 16 + (lane >> 2) + 8 * h) * 64 + 8 * i + 2 * (lane & 3) + e] = d[4 * i + 2 * h + e];
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) { tc_fence_after(); tmem_dealloc(tmem, 64); }
 }
 
 }  // namespace ctpn
@@ -91,288 +77,6 @@ extern "C" int ctpn_probe_umma_view(const void *a, const void *ident, int rows, 
   const size_t smem = 1024 + (size_t)((rows * 128 + 1023) & ~1023) + 64 * 128;
   CTPN_CUDA(cudaFuncSetAttribute(probe_umma_view_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   probe_umma_view_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(ta, tb, rows, row0, group_stride_rows, base_offset_mode, out);
-  CTPN_LAUNCH_CHECK();
-  return CTPN_OK;
-}
-
-// ---- probe 2: sustained tcgen05.mma issue rate vs commit / barrier-wait cadence ------------------
-// Every CTA (one per SM) issues `n_mma` 128 x BN x 16 bf16 MMAs on a fixed (zeroed) shared-memory tile,
-// with a tcgen05.commit every `commit_every` MMAs and, optionally, a wait on that commit's mbarrier
-// `lag` commits later (lag 0 = never wait until the end).  Answers: does a commit stall the tensor pipe?
-namespace ctpn {
-
-template <int BN>
-__global__ void __launch_bounds__(128, 1)
-probe_mma_rate_kernel(int n_mma, int commit_every, int lag, int alternate_acc, int fence_each) {
-  using namespace ptx;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sa = (raw + 1023u) & ~1023u, sb = sa + 16384;
-  __shared__ uint64_t bars[64];
-  __shared__ uint32_t tmem_slot;
-  for (int i = threadIdx.x; i < (16384 + BN * 128) / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem_raw + (sa - raw))[i] = 0;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 64; ++i) mbar_init(smem_u32(&bars[i]), 1);
-    fence_mbar_init();
-  }
-  fence_proxy_async();
-  if (threadIdx.x < 32) { tmem_alloc(smem_u32(&tmem_slot), 512); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  if (__shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0) == 0) {   // whole warp, uniform control flow
-    const uint32_t idesc = umma_idesc_bf16(128, BN);
-    const uint64_t da = umma_desc_k_sw128(sa), db = umma_desc_k_sw128(sb);
-    int commits = 0, waited = 0;
-    if (fence_each == 2) {   // tight mode: 8 back-to-back MMAs per elected region, no per-MMA warp sync
-      for (int i = 0; i < n_mma; i += 8) {
-        if (elect_one()) {
-#pragma unroll
-          for (int u = 0; u < 8; ++u) mma_bf16_ss(tmem + ((alternate_acc && (u & 4)) ? BN : 0), da + 2ull * (u & 3), db + 2ull * (u & 3), idesc, (i | u) > 7);
-        }
-        __syncwarp();
-      }
-    } else
-    for (int i = 0; i < n_mma; ++i) {
-      const uint32_t d = tmem + ((alternate_acc && (i & 4)) ? BN : 0);
-      if (elect_one()) mma_bf16_ss(d, da + 2ull * (i & 3), db + 2ull * (i & 3), idesc, i > 7);
-      __syncwarp();
-      if ((i + 1) % commit_every == 0) {
-        if (elect_one()) mma_commit(smem_u32(&bars[commits & 31]));
-        __syncwarp();
-        ++commits;
-        if (lag > 0 && commits - waited > lag) {
-          mbar_wait(smem_u32(&bars[waited & 31]), (waited >> 5) & 1);
-          if (fence_each) tc_fence_after();
-          ++waited;
-        }
-      }
-    }
-    if (lag > 0)
-      while (waited < commits) { mbar_wait(smem_u32(&bars[waited & 31]), (waited >> 5) & 1); ++waited; }
-    if (elect_one()) mma_commit(smem_u32(&bars[40]));      // final: everything issued so far has completed
-    __syncwarp();
-    mbar_wait(smem_u32(&bars[40]), 0);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) { tc_fence_after(); tmem_dealloc(tmem, 512); }
-}
-
-
-// ---- CTA-pair (cta_group::2) dispatch-rate probe: one instruction drives the tensor cores of both SMs of a
-// 2-CTA cluster (M = 256: 128 rows per CTA; each CTA holds its A rows and half of B's N rows). ----
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(128, 1)
-probe_mma_rate_pair_kernel(int n_mma, int alternate_acc) {
-  using namespace ptx;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sa = (raw + 1023u) & ~1023u, sb = sa + 16384;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  for (int i = threadIdx.x; i < (16384 + BN * 64) / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem_raw + (sa - raw))[i] = 0;
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bar), 1);
-    fence_mbar_init();
-  }
-  fence_proxy_async();
-  cluster_sync_all();
-  if (threadIdx.x < 32) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const bool leader = ptx::cluster_ctarank() == 0;
-  if (__shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0) == 0) {
-    if (leader) {
-      const uint32_t idesc = umma_idesc_bf16(256, BN);
-      const uint64_t da = umma_desc_k_sw128(sa), db = umma_desc_k_sw128(sb);
-      for (int i = 0; i < n_mma; i += 8) {
-        if (elect_one()) {
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const uint32_t d = tmem + ((alternate_acc && (u & 4)) ? BN : 0);
-            const uint32_t acc = (i | u) > 7;
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t"
-                "setp.ne.b32 p, %4, 0;\n\t"
-                "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                ::"r"(d), "l"(da + 2ull * (u & 3)), "l"(db + 2ull * (u & 3)), "r"(idesc), "r"(acc)
-                : "memory");
-          }
-        }
-        __syncwarp();
-      }
-      if (elect_one())   // arrive on the barrier at this offset in BOTH CTAs once every MMA above has completed
-        asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                     ::"r"(smem_u32(&bar)), "h"((uint16_t)3) : "memory");
-      __syncwarp();
-    }
-    mbar_wait(smem_u32(&bar), 0);
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (threadIdx.x < 32) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-  }
-}
-
-}  // namespace ctpn
-
-// ---- probe 3: dispatch rate of kind::f8f6f4 (e4m3, K = 32 per instruction) next to kind::f16 (K = 16), from one CTA
-// (M = 128) or a CTA pair (cta_group::2, M = 256).  mode 0: all f16; 1: all f8; 2: groups of 4 f16 -> accumulator 0 followed
-// by 4 f8 -> accumulator 1 (the issue pattern of a "fp16 main + fp8 cross" convolution step).  Same operand bytes per
-// instruction for both kinds (128 rows x 32 B of A), so the comparison isolates the tensor-pipe rate.
-namespace ctpn {
-
-template <int BN, int PAIR, int MODE>
-__global__ void __launch_bounds__(128, 1)
-probe_mma_kind_kernel(int n_mma) {
-  constexpr int mode = MODE;     // compile time: the unrolled issue loop has no branches
-  using namespace ptx;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t sa = (raw + 1023u) & ~1023u, sb = sa + 16384;
-  constexpr int kBRows = PAIR ? BN / 2 : BN;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
-  for (int i = threadIdx.x; i < (16384 + kBRows * 128) / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem_raw + (sa - raw))[i] = 0;
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(&bar), 1);
-    fence_mbar_init();
-  }
-  fence_proxy_async();
-  if (PAIR) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x < 32) {
-    if (PAIR) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512u) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      tmem_alloc(smem_u32(&tmem_slot), 512);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const bool leader = !PAIR || cluster_ctarank() == 0;
-  if (__shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0) == 0) {
-    if (leader) {
-      constexpr int M = PAIR ? 256 : 128;
-      const uint32_t id16 = umma_idesc_bf16(M, BN), id8 = umma_idesc_e4m3(M, BN);
-      const uint64_t da = umma_desc_k_sw128(sa), db = umma_desc_k_sw128(sb);
-      const uint32_t acc1 = (2 * BN <= 512) ? (uint32_t)BN : 0u;
-      for (int i = 0; i < n_mma; i += 8) {
-        if (elect_one()) {
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            const bool f8 = mode == 1 || (mode == 2 && (u & 4));
-            const uint32_t d = tmem + ((mode == 2 && (u & 4)) ? acc1 : 0u);
-            const uint32_t acc = (i | u) > 7;
-            const uint64_t a = da + 2ull * (u & 3), b = db + 2ull * (u & 3);
-            if (PAIR) {
-              if (f8) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-                                   ::"r"(d), "l"(a), "l"(b), "r"(id8), "r"(acc) : "memory");
-              else asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                                ::"r"(d), "l"(a), "l"(b), "r"(id16), "r"(acc) : "memory");
-            } else {
-              if (f8) asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-                                   ::"r"(d), "l"(a), "l"(b), "r"(id8), "r"(acc) : "memory");
-              else asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                                ::"r"(d), "l"(a), "l"(b), "r"(id16), "r"(acc) : "memory");
-            }
-          }
-        }
-        __syncwarp();
-      }
-      if (elect_one()) {
-        if (PAIR) asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                               ::"r"(smem_u32(&bar)), "h"((uint16_t)3) : "memory");
-        else mma_commit(smem_u32(&bar));
-      }
-      __syncwarp();
-    }
-    mbar_wait(smem_u32(&bar), 0);
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();
-  if (threadIdx.x < 32) {
-    tc_fence_after();
-    if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-    else tmem_dealloc(tmem, 512);
-  }
-}
-
-}  // namespace ctpn
-
-extern "C" int ctpn_probe_mma_kind(int bn, int pair, int mode, int n_mma, int grid, void *stream) {
-  CTPN_REQUIRE(bn == 64 || bn == 128 || bn == 256, "ctpn_probe_mma_kind: bn must be 64/128/256");
-  CTPN_REQUIRE(n_mma > 0 && n_mma % 8 == 0 && grid > 0 && mode >= 0 && mode <= 2, "ctpn_probe_mma_kind: bad arguments");
-  CTPN_REQUIRE(!pair || grid % 2 == 0, "ctpn_probe_mma_kind: pair mode needs an even grid");
-  const size_t smem = 1024 + 16384 + (size_t)bn * (pair ? 64 : 128);
-  cudaStream_t st = (cudaStream_t)stream;
-#define CTPN_LAUNCH_KIND(BN, PAIR)                                                                                 \
-  do {                                                                                                             \
-    auto k = mode == 0 ? probe_mma_kind_kernel<BN, PAIR, 0> : mode == 1 ? probe_mma_kind_kernel<BN, PAIR, 1> : probe_mma_kind_kernel<BN, PAIR, 2>; \
-    CTPN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                    \
-    cudaLaunchConfig_t cfg = {};                                                                                   \
-    cudaLaunchAttribute attr;                                                                                      \
-    attr.id = cudaLaunchAttributeClusterDimension;                                                                 \
-    attr.val.clusterDim.x = PAIR ? 2 : 1; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;                    \
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(128); cfg.dynamicSmemBytes = smem; cfg.stream = st;              \
-    cfg.attrs = &attr; cfg.numAttrs = 1;                                                                           \
-    CTPN_CUDA(cudaLaunchKernelEx(&cfg, k, n_mma));                                                           \
-  } while (0)
-  if (pair) {
-    if (bn == 256) CTPN_LAUNCH_KIND(256, 1); else if (bn == 128) CTPN_LAUNCH_KIND(128, 1); else CTPN_LAUNCH_KIND(64, 1);
-  } else {
-    if (bn == 256) CTPN_LAUNCH_KIND(256, 0); else if (bn == 128) CTPN_LAUNCH_KIND(128, 0); else CTPN_LAUNCH_KIND(64, 0);
-  }
-#undef CTPN_LAUNCH_KIND
-  CTPN_LAUNCH_CHECK();
-  return CTPN_OK;
-}
-
-extern "C" int ctpn_probe_mma_rate(int bn, int n_mma, int commit_every, int lag, int alternate_acc, int fence_each,
-                                   int grid, void *stream) {
-  CTPN_REQUIRE(bn == 64 || bn == 128 || bn == 256, "ctpn_probe_mma_rate: bn must be 64/128/256");
-  CTPN_REQUIRE(n_mma > 0 && commit_every > 0 && lag >= 0 && lag < 32 && grid > 0, "ctpn_probe_mma_rate: bad arguments");
-  const size_t smem = 1024 + 16384 + (size_t)bn * 128;
-  cudaStream_t st = (cudaStream_t)stream;
-#define CTPN_LAUNCH_PROBE(BN)                                                                                      \
-  do {                                                                                                             \
-    CTPN_CUDA(cudaFuncSetAttribute(probe_mma_rate_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    probe_mma_rate_kernel<BN><<<grid, 128, smem, st>>>(n_mma, commit_every, lag, alternate_acc, fence_each);       \
-  } while (0)
-  if (bn == 256) CTPN_LAUNCH_PROBE(256);
-  else if (bn == 128) CTPN_LAUNCH_PROBE(128);
-  else CTPN_LAUNCH_PROBE(64);
-#undef CTPN_LAUNCH_PROBE
-  CTPN_LAUNCH_CHECK();
-  return CTPN_OK;
-}
-
-extern "C" int ctpn_probe_mma_rate_pair(int bn, int n_mma, int alternate_acc, int grid, void *stream) {
-  CTPN_REQUIRE(bn == 64 || bn == 128 || bn == 256, "ctpn_probe_mma_rate_pair: bn must be 64/128/256");
-  CTPN_REQUIRE(n_mma > 0 && n_mma % 8 == 0 && grid > 0 && grid % 2 == 0, "ctpn_probe_mma_rate_pair: bad arguments");
-  const size_t smem = 1024 + 16384 + (size_t)bn * 64;
-  cudaStream_t st = (cudaStream_t)stream;
-#define CTPN_LAUNCH_PROBE(BN)                                                                                      \
-  do {                                                                                                             \
-    CTPN_CUDA(cudaFuncSetAttribute(probe_mma_rate_pair_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    probe_mma_rate_pair_kernel<BN><<<grid, 128, smem, st>>>(n_mma, alternate_acc);                                 \
-  } while (0)
-  if (bn == 256) CTPN_LAUNCH_PROBE(256);
-  else if (bn == 128) CTPN_LAUNCH_PROBE(128);
-  else CTPN_LAUNCH_PROBE(64);
-#undef CTPN_LAUNCH_PROBE
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
 }

@@ -1,4 +1,4 @@
-"""ctpn_b200: B200-native CTPN text-detection hot path (drop-in for the detection path of
+"""ctpn_b200: H100-native (sm_90a) CTPN text-detection hot path (drop-in for the detection path of
 eragonruan/text-detection-ctpn).  Importing the package loads libctpn_b200.so; there is no
 CPU fallback."""
 from ._native import CtpnError, LIB_PATH, lib  # noqa: F401

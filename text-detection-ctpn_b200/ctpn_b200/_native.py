@@ -78,9 +78,6 @@ SIGNATURES = {
 TESTING_SIGNATURES = {
     "ctpn_conv1_1": (_i, [_p, _i, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "ctpn_conv3x3_simt": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
-    "ctpn_probe_mma_rate": (_i, [_i, _i, _i, _i, _i, _i, _i, _p]),
-    "ctpn_probe_mma_rate_pair": (_i, [_i, _i, _i, _i, _p]),
-    "ctpn_probe_mma_kind": (_i, [_i, _i, _i, _i, _i, _p]),
     "ctpn_probe_umma_view": (_i, [_p, _p, _i, _i, _i, _i, _p, _p]),
 }
 

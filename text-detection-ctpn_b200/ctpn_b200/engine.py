@@ -1,4 +1,4 @@
-"""Engine: host-side driver of the B200 CTPN hot path.
+"""Engine: host-side driver of the H100 CTPN hot path.
 
 PyTorch is used only as plumbing (device memory, streams, pinned buffers); all
 compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
@@ -38,7 +38,7 @@ class Engine:
         self.graph_max_batch = int(graph_max_batch)
         self._graphs = {}
         if not torch.cuda.is_available():
-            raise N.CtpnError("ctpn_b200.Engine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise N.CtpnError("ctpn_b200.Engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         torch.cuda.set_device(self.device)
         N.check(N.lib.ctpn_device_ok(device), "ctpn_device_ok")

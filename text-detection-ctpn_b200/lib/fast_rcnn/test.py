@@ -1,5 +1,5 @@
 """test_ctpn(sess, net, im) -> (scores, boxes): the inference entry point of
-lib/fast_rcnn/test.py:40-58, same signature and results, running on the B200 engine.
+lib/fast_rcnn/test.py:40-58, same signature and results, running on the H100 engine.
 
 Host pre-processing follows test.py:7-31 (float32 copy, mean subtraction, rescale to
 TEST.SCALES / TEST.MAX_SIZE with cv2.INTER_LINEAR).  When no rescale is needed and the image is

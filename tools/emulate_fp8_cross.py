@@ -6,7 +6,7 @@ Every 3x3 layer is evaluated as  main + cross  with
   main  = conv(a0, w0)                                   a0 = bf16(a), w0 = bf16(w)         (exact products, f32/f64 sum)
   cross = conv(q(a0), q(w1)) + conv(q(a1), q(w0))        a1 = bf16(a - a0), w1 = bf16(w - w0)
 where q() is bf16 (today's 3-MMA mode) or e4m3 with a per-tensor power-of-two scale (the proposed 2-unit mode:
-kind::f8f6f4 MMAs run at twice the bf16 rate).  The BiLSTM / FC / heads stay float32.  Compared against the float64
+e4m3 MMAs run at twice the bf16 rate).  The BiLSTM / FC / heads stay float32.  Compared against the float64
 evaluation of the float32 model on one synthetic 600x900 image.
 
     python tools/emulate_fp8_cross.py [--height 600 --width 900 --seed 0]

@@ -3,7 +3,7 @@
 written as the JSON bench.py reads for roofline.traffic.  The file is stamped with the SHA-256 of the kernel sources it was
 captured from (bench.py refuses it when the sources have changed since).
 
-    python tools/ncu_traffic.py gpurun_out/r2h/ncu_raw_f16f8.csv --config 2 --mode f16f8 --batch 32 > profiles/r2_conv_traffic_cfg2_f16f8.json
+    python tools/ncu_traffic.py ncu_raw_f16f8.csv --config 2 --mode f16f8 --batch 32 > profiles/conv_traffic_cfg2_f16f8.json
 """
 import argparse
 import csv

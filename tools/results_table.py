@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Markdown table of the committed bench lines (profiles/r2_bench_*.json), pasted into DESIGN.md section 6.
+"""Markdown table of bench JSON lines (files holding bench.py output).
 
-    python tools/results_table.py profiles/r2_bench_cfg2.json profiles/r2_bench_cfg3.json ...
+    python tools/results_table.py bench_cfg2.json bench_cfg3.json ...
 """
 import json
 import sys
