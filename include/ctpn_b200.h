@@ -124,6 +124,12 @@ int ctpn_conv1_1_tc(const void *src, int src_is_f32, const float *lut, const flo
  * stacked layout [B][Ho + 1][Wo] -- a STACK_IN layer also writes the zero rows, a plain-input layer leaves them to the caller. */
 #define CTPN_F_STACK_IN 16
 #define CTPN_F_STACK_OUT 32
+/* PROMOTE (ctpn_conv3x3 with planes = 3 only; CTPN_ERR_INVALID otherwise and on ctpn_conv3x3_f16f8): the tensor core truncates
+ * when it adds a K=16 partial sum into a float32 accumulator, and over the 9 * Cin / 16 adds of a 512-channel layer those
+ * truncations add up to ~10x the error of float32 with round-to-nearest (DESIGN.md section 5).  With this flag the plane-0 x
+ * plane-0 accumulator restarts every 64 channels of one tap and its partial sums are added with round-to-nearest float32
+ * adds; the cross-plane terms (2^-8 smaller) accumulate as before. */
+#define CTPN_F_PROMOTE 64
 int ctpn_conv3x3(const void *in_planes, const void *w_planes, const float *bias, void *out, int B,
                  int H, int W, int cin, int cout, int taps, int planes, int flags, void *stream);
 /* The same layers in the "F16F8" arithmetic: 2 tensor-core units per MAC instead of the 3 of two bf16 planes; head logits
@@ -153,10 +159,13 @@ int ctpn_bilstm_recurrent(const float *xproj, const float *wh_fw, const float *w
 
 /* ---- whole network up to the head tensors -------------------------------------------- */
 typedef struct ctpn_net ctpn_net_t;
-/* planes: 1..3 bf16 planes, or CTPN_ARITH_F16F8: conv1_1 + the thirteen 3x3 layers in the 2-unit F16F8 arithmetic (the
+/* planes: 1..3 bf16 planes, CTPN_ARITH_BF16X3P, or CTPN_ARITH_F16F8: conv1_1 + the thirteen 3x3 layers in the 2-unit F16F8 arithmetic (the
  * matmuls around the BiLSTM stay on two bf16 planes).  F16F8 activation scales are calibrated on the first batch that
- * ctpn_net_forward sees and then frozen (option "recalibrate" re-arms the calibration). */
+ * ctpn_net_forward sees and then frozen (option "recalibrate" re-arms the calibration).
+ * CTPN_ARITH_BF16X3P: three bf16 planes (as planes = 3) with CTPN_F_PROMOTE on the thirteen 3x3 layers and the three matmuls
+ * (x-projection, FC, heads); conv1_1 (K = 32, one two-MMA chain) and the BiLSTM are the same as with planes = 3. */
 #define CTPN_ARITH_F16F8 4
+#define CTPN_ARITH_BF16X3P 5
 int ctpn_net_create(ctpn_net_t **net, int planes);
 int ctpn_net_destroy(ctpn_net_t *net);
 /* options: "keep_activations" (1: every layer gets its own workspace region so that

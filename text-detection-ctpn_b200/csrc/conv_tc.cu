@@ -71,6 +71,7 @@ struct ConvTcParams {
   int in_stack_h, out_rows, out_stacked;
   double work;              // algorithmic FLOPs of the call (profiling label only)
   int stage_small;          // 1: 512-byte store-transpose block per epilogue warp (8 pixels per round)
+  int promote_every;        // test library only (CTPN_TC_PROMOTE): pipeline steps per promoted main chain (product: 1)
 };
 
 constexpr int kTcThreads = 384;   // warpgroup 0: producers (warp 0 weights, warp 1 activations); 1 and 2: MMAs + epilogue
@@ -87,13 +88,18 @@ constexpr int kEpiBytes = 2 * 128 * 32 * 4;        // float32 staging of two 32-
 // F8 = 1 (with P = 2 stage slots): the F16F8 arithmetic -- plane 0 holds fp16 operands (fp16 wgmma into the main
 // accumulator), plane 1 the K-concatenated e4m3 copies (e4m3 wgmma, K = 32, into the cross accumulator): 4 + 4 tensor
 // core instructions per (tap, channel block) where two bf16 planes need 12.
-template <int BN, int P, int TAPS, int MC, int F8>
+// PR = 1 (CTPN_F_PROMOTE, P = 3 only): the main accumulator is restarted at every pipeline step (one tap of one channel
+// block, K = 64) and each step's partial sum is added into a third register array with round-to-nearest float32 adds, so
+// the tensor core's truncating adds run over chains of 4 MMAs instead of 4 * 9 * Cin / 64.  Each step commits its main and
+// its cross MMAs as two groups; the promotion waits for the main group only and overlaps the cross MMAs.
+template <int BN, int P, int TAPS, int MC, int F8, int PR = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const ConvTcParams p) {
   using namespace ptx;
   constexpr int kBBytes = BN * 128;
   static_assert(!F8 || P == 2, "F16F8 uses two stage slots per operand");
+  static_assert(!PR || (P == 3 && !F8), "promotion is built for three bf16 planes");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t ring_a = (raw + 1023u) & ~1023u;
@@ -197,6 +203,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const bool leader = (threadIdx.x & 127) == 0;
     constexpr int R = BN / 2;                  // accumulator registers per thread (64 x BN per warpgroup)
     float accm[R], accc[R];                    // main and (P > 1) cross accumulators
+    float accs[R];                             // PR: round-to-nearest sum of the promoted main chains (unused otherwise)
+#ifdef CTPN_DEBUG
+    const int pe = PR ? p.promote_every : 1;   // steps per main chain
+#else
+    constexpr int pe = 1;
+#endif
     // Descriptors are (per-stage low word) + compile-time offsets: planes, taps and k-slices are fully unrolled.
     constexpr uint32_t kPatch16 = (TAPS == 9 ? 23552u : 16384u) >> 4;   // plane stride of the A stage, in 16-B units
     constexpr uint32_t kB16 = (uint32_t)kBBytes >> 4;
@@ -224,6 +236,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
     };
     for (int u = u_begin; u < p.total_units; u += u_step) {
+      if (PR) {
+#pragma unroll
+        for (int i = 0; i < R; ++i) accs[i] = 0.f;
+      }
       for (int kb = 0; kb < kblocks; ++kb) {
         if (p.stages_a == 1 && prev_a >= 0) {   // a single activation stage: it must be free before its next load
           wgmma_wait<0>();
@@ -239,6 +255,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           constexpr int kPW = 10;
           const uint32_t view16 = TAPS == 9 ? (uint32_t)((tap / 3) * kPW + tap % 3) * 8u : 0u;
           const uint32_t not_first = (kb | tap) != 0;
+          const int step = kb * TAPS + tap;
           wgmma_fence();
           if (!CTPN_DBG(p, 4)) {
             if (F8) {
@@ -250,6 +267,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
               for (int k = 0; k < 4; ++k)     // e4m3 x e4m3, K = 32 (32 B): k 0,1 = value x residual, k 2,3 = residual x value
                 wgmma_e4m3(accc, ((uint64_t)hi_a << 32) | (a_lo + kPatch16 + view16 + 2u * k),
                            ((uint64_t)kHiB << 32) | (b_lo + kB16 + 2u * k), k == 0 ? not_first : 1u);
+            } else if (PR) {
+              const uint32_t chain_on = step % pe != 0;     // 0: this step starts a new main chain
+#pragma unroll
+              for (int k = 0; k < 4; ++k)
+                wgmma_bf16(accm, ((uint64_t)hi_a << 32) | (a_lo + view16 + 2u * k), ((uint64_t)kHiB << 32) | (b_lo + 2u * k),
+                           k == 0 ? chain_on : 1u);
+              wgmma_commit();                               // the main group: the promotion below waits for it alone
+#pragma unroll
+              for (int i = 0; i < P; ++i) {
+#pragma unroll
+                for (int j = (i == 0); j < P - i; ++j) {
+#pragma unroll
+                  for (int k = 0; k < 4; ++k) {
+                    const uint64_t da = ((uint64_t)hi_a << 32) | (a_lo + i * kPatch16 + view16 + 2u * k);
+                    const uint64_t db = ((uint64_t)kHiB << 32) | (b_lo + j * kB16 + 2u * k);
+                    wgmma_bf16(accc, da, db, (k == 0 && i == 0 && j == 1) ? not_first : 1u);
+                  }
+                }
+              }
             } else {
 #pragma unroll
               for (int i = 0; i < P; ++i) {
@@ -267,10 +303,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
             }
           }
           wgmma_commit();
-          wgmma_wait<1>();                   // the previous step's MMAs are done: free its stages
+          // the previous step's MMAs are done: free its stages (PR: groups retire in order, so this step's main group is done too)
+          wgmma_wait<1>();
           if (prev_b >= 0) release(prev_b, prev_a);
           prev_b = sb;
           prev_a = tap == TAPS - 1 ? sa : -1;
+          if (PR && ((step + 1) % pe == 0 || step == kblocks * TAPS - 1)) {
+            wgmma_fence_regs(accm);
+#pragma unroll
+            for (int i = 0; i < R; ++i) accs[i] = __fadd_rn(accs[i], accm[i]);   // (0 + x is exact)
+          }
           if (++sb == p.stages_b) { sb = 0; phb ^= 1u; }
         }
         if (++sa == p.stages_a) { sa = 0; pha ^= 1u; }
@@ -283,7 +325,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       // main (+ cross): kept apart during the K loop because the tensor core truncates when it adds into float32
       if (P > 1) {
 #pragma unroll
-        for (int i = 0; i < R; ++i) accm[i] = F8 ? __fmaf_rn(accc[i], p.inv_cross, accm[i] * p.inv_main) : accm[i] + accc[i];
+        for (int i = 0; i < R; ++i)
+          accm[i] = F8 ? __fmaf_rn(accc[i], p.inv_cross, accm[i] * p.inv_main) : PR ? __fadd_rn(accs[i], accc[i]) : accm[i] + accc[i];
       }
 
       // ===== epilogue: +bias -> ReLU -> optional fused 2x2 max-pool (warp shuffles: the window of a pixel lives in lanes
@@ -494,7 +537,7 @@ constexpr int kMaxDevices = 64;
 static std::mutex g_mu;
 static int g_sms[kMaxDevices];
 
-struct Tuning { int debug = 0, bn = 0, stages_a = 0, stages_b = 0, mcast = 1, stage_small = 1; };
+struct Tuning { int debug = 0, bn = 0, stages_a = 0, stages_b = 0, mcast = 1, stage_small = 1, promote = 1; };
 static const Tuning &tuning() {            // read once at first use; overrides exist only in the test library
   static const Tuning t = [] {
     Tuning v;
@@ -506,6 +549,7 @@ static const Tuning &tuning() {            // read once at first use; overrides 
     v.stages_b = env_int("CTPN_TC_STAGES_B", 0);
     v.mcast = env_int("CTPN_TC_MCAST", 1);
     v.stage_small = env_int("CTPN_TC_STAGE_SMALL", 1);
+    v.promote = std::max(1, env_int("CTPN_TC_PROMOTE", 1));   // CTPN_F_PROMOTE: pipeline steps per promoted main chain
 #endif
     return v;
   }();
@@ -550,7 +594,7 @@ static int cached_tmap(int dev, CUtensorMap *out, const void *ptr, int rank, con
   return CTPN_OK;
 }
 
-template <int BN, int P, int TAPS, int MC, int F8 = 0>
+template <int BN, int P, int TAPS, int MC, int F8 = 0, int PR = 0>
 static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, ConvTcParams &p, cudaStream_t st) {
   const size_t a_stage = (size_t)p.planes * p.patch_bytes, b_stage = (size_t)p.planes * BN * 128;
   // long-K F16F8 layers store through 8-pixel rounds (a 512-byte transpose block per warp)
@@ -570,7 +614,7 @@ static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, Conv
   p.stages_b = sb;
   const size_t smem = 1024 + sa * a_stage + sb * b_stage + kEpiBytes + kCtrlBytes;
   CTPN_REQUIRE(smem <= 227 * 1024, "conv_tc: %zu bytes of shared memory", smem);
-  auto kernel = conv_tc_kernel<BN, P, TAPS, MC, F8>;
+  auto kernel = conv_tc_kernel<BN, P, TAPS, MC, F8, PR>;
   static bool attr_set[kMaxDevices];
   static int max_clusters[kMaxDevices];     // co-resident 2-CTA clusters of this instantiation (one CTA per SM)
   cudaLaunchConfig_t cfg = {};
@@ -597,7 +641,7 @@ static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, Conv
     }
   }
   char label[128];
-  if (prof_enabled()) snprintf(label, sizeof(label), "conv_tc t%d %dx%dx%d c%d-%d %s%d bn%d%s", p.taps, p.B, p.H, p.W, p.Cin, p.Cout, F8 ? "f16f8 p" : "p", p.planes, BN, MC ? " mc" : "");
+  if (prof_enabled()) snprintf(label, sizeof(label), "conv_tc t%d %dx%dx%d c%d-%d %s%d bn%d%s%s", p.taps, p.B, p.H, p.W, p.Cin, p.Cout, F8 ? "f16f8 p" : "p", p.planes, BN, MC ? " mc" : "", PR ? " promote" : "");
   ProfScope prof(label, p.work, st);
   if (MC) cfg.gridDim = dim3(2 * std::min(max_clusters[dev], p.total_units));
   else cfg.gridDim = dim3(std::min(p.total_units, g_sms[dev]));
@@ -615,7 +659,9 @@ struct QuantScales { float inv_main, inv_cross, out_s, out_t; };
 
 static int conv_tc_run(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
                        int cout, int taps, int planes, int flags, const QuantScales *q, void *stream) {
-  const bool f8 = q != nullptr;
+  const bool f8 = q != nullptr, promote = (flags & CTPN_F_PROMOTE) != 0;
+  CTPN_REQUIRE(!(promote && f8), "ctpn_conv3x3_f16f8: CTPN_F_PROMOTE is a flag of ctpn_conv3x3 with planes = 3");
+  CTPN_REQUIRE(!promote || planes == 3, "ctpn_conv3x3: CTPN_F_PROMOTE needs planes = 3 (got %d)", planes);
   CTPN_REQUIRE(in_planes && w_planes && bias && out, "ctpn_conv3x3: null pointer");
   CTPN_REQUIRE(taps == 9 || taps == 1, "ctpn_conv3x3: taps must be 9 or 1 (got %d)", taps);
   CTPN_REQUIRE(planes >= 1 && planes <= 3, "ctpn_conv3x3: planes must be 1..3 (got %d)", planes);
@@ -676,6 +722,7 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
     p.out_rs = kResidualGain * q->out_t / q->out_s;
   }
   p.debug = tuning().debug;
+  p.promote_every = tuning().promote;
 
   // N tile: 256 halves the A traffic per MAC; with two accumulators per tile (P > 1) it would need 256 accumulator
   // registers per consumer thread, so those stay at 128.
@@ -683,14 +730,17 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   if (!(BN == 64 || BN == 128 || BN == 256)) BN = 256;
   if (planes > 1 && BN > 128) BN = 128;   // main + cross accumulators: 2 * BN / 2 registers per thread (F16F8 too)
   while (BN > cout || cout % BN) BN >>= 1;
-  p.tiles_n = cout / BN;
   const long long m_tiles = (long long)B * p.tiles_x * p.tiles_y;
+  // weight-tile multicast over 2-CTA clusters (3x3 layers with at least one pair of pixel tiles per SM pair)
+  const bool mc = taps == 9 && tuning().mcast != 0 && m_tiles >= 2;
+  // promoted single-CTA 3x3 layers (a map of one 16 x 8 tile) run at BN = 64: with three accumulators that kernel
+  // spills registers at BN = 128, the multicast and taps = 1 ones do not
+  if (promote && taps == 9 && !mc && BN > 64) BN = 64;
+  p.tiles_n = cout / BN;
   const long long total = m_tiles * p.tiles_n;
   CTPN_REQUIRE(total < (1ll << 31), "ctpn_conv3x3: too many tiles");
   p.total_tiles = (int)total;
   p.m_tiles = (int)m_tiles;
-  // weight-tile multicast over 2-CTA clusters (3x3 layers with at least one pair of pixel tiles per SM pair)
-  const bool mc = taps == 9 && tuning().mcast != 0 && m_tiles >= 2;
   p.total_units = mc ? (int)((m_tiles + 1) / 2) * p.tiles_n : p.total_tiles;
 
   CUtensorMap ta, tb;
@@ -720,6 +770,15 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
     if (taps == 1 && BN == 128) return launch_bn<128, 2, 1, 0, 1>(dev, ta, tb, p, st);
     if (taps == 1 && BN == 64) return launch_bn<64, 2, 1, 0, 1>(dev, ta, tb, p, st);
     set_error("ctpn_conv3x3_f16f8: no kernel for BN=%d taps=%d", BN, taps);
+    return CTPN_ERR_INVALID;
+  }
+  if (promote) {   // planes == 3
+    if (mc && BN == 128) return launch_bn<128, 3, 9, 1, 0, 1>(dev, ta, tb, p, st);
+    if (mc && BN == 64) return launch_bn<64, 3, 9, 1, 0, 1>(dev, ta, tb, p, st);
+    if (taps == 9 && BN == 64) return launch_bn<64, 3, 9, 0, 0, 1>(dev, ta, tb, p, st);
+    if (taps == 1 && BN == 128) return launch_bn<128, 3, 1, 0, 0, 1>(dev, ta, tb, p, st);
+    if (taps == 1 && BN == 64) return launch_bn<64, 3, 1, 0, 0, 1>(dev, ta, tb, p, st);
+    set_error("ctpn_conv3x3: no promoted kernel for BN=%d taps=%d", BN, taps);
     return CTPN_ERR_INVALID;
   }
   CTPN_TC_CASE_MC(256, 1); CTPN_TC_CASE_MC(128, 1); CTPN_TC_CASE_MC(64, 1);

@@ -42,6 +42,7 @@ struct ctpn_net {
   // BiLSTM (0.9 % of the FLOPs) stay on two bf16 planes.  Per-layer power-of-two scales: w_s / w_t from max|w| at
   // finalize time; act_s / act_t (quantisation of the layer's OUTPUT) from the first batch seen (calibrate()).
   bool f16f8 = false, calibrated = false;
+  bool promote = false;     // CTPN_ARITH_BF16X3P: planes = 3 with CTPN_F_PROMOTE on every conv_tc layer
   float w_s[14] = {0}, w_t[14] = {0}, act_s[14] = {0}, act_t[14] = {0}, act_max[14] = {0};
   unsigned *absmax_dev = nullptr;
   int conv_simt = 0, conv1_simt = 0, keep = 0;
@@ -343,10 +344,12 @@ static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, int 
 
 extern "C" int ctpn_net_create(ctpn_net_t **net, int planes) {
   CTPN_REQUIRE(net, "ctpn_net_create: null pointer");
-  CTPN_REQUIRE((planes >= 1 && planes <= 3) || planes == CTPN_ARITH_F16F8, "ctpn_net_create: planes must be 1..3 or CTPN_ARITH_F16F8 (got %d)", planes);
+  CTPN_REQUIRE((planes >= 1 && planes <= 3) || planes == CTPN_ARITH_F16F8 || planes == CTPN_ARITH_BF16X3P,
+               "ctpn_net_create: planes must be 1..3, CTPN_ARITH_F16F8 or CTPN_ARITH_BF16X3P (got %d)", planes);
   ctpn_net *n = new ctpn_net();
   n->f16f8 = planes == CTPN_ARITH_F16F8;
-  n->planes = n->f16f8 ? 2 : planes;
+  n->promote = planes == CTPN_ARITH_BF16X3P;
+  n->planes = n->f16f8 ? 2 : n->promote ? 3 : planes;
   *net = n;
   return CTPN_OK;
 }
@@ -429,13 +432,14 @@ extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_
   auto conv1 = ctpn_conv1_1_tc;
   auto conv3 = ctpn_conv3x3;
 #endif
+  const int pf = net->promote ? CTPN_F_PROMOTE : 0;     // CTPN_ARITH_BF16X3P: every conv_tc layer below
   if (!net->f16f8) {
   if ((rc = conv1(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, P, stream))) return rc;
   net->taps["conv1_1"] = Tap{ws + L.act[0], (long long)B * H * W, 64, true};
   int h = H, w = W;
   for (int l = 1; l < 14; ++l) {
     const ConvSpec &s = kConvs[l];
-    int flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0);
+    int flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0) | pf;
     const bool stacked = L.stack && l >= 9 && l <= 12;
     if (stacked) flags |= CTPN_F_STACK_OUT;
     if (L.stack && l >= 10) flags |= CTPN_F_STACK_IN;
@@ -449,13 +453,13 @@ extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_
   }
   const int M = B * L.fh * L.fw;
   auto gemm = conv3;
-  if ((rc = gemm(ws + L.act[13], net->xproj_w, net->xproj_b, ws + L.xproj, 1, 1, M, 512, 1024, 1, P, CTPN_F_OUT_F32, stream))) return rc;
+  if ((rc = gemm(ws + L.act[13], net->xproj_w, net->xproj_b, ws + L.xproj, 1, 1, M, 512, 1024, 1, P, CTPN_F_OUT_F32 | pf, stream))) return rc;
   net->taps["xproj"] = Tap{ws + L.xproj, M, 1024, false};
   if ((rc = ctpn_bilstm_recurrent((const float *)(ws + L.xproj), net->wh_fw, net->wh_bw, ws + L.act[14], B * L.fh, L.fw, P, stream))) return rc;
   net->taps["lstm_out"] = Tap{ws + L.act[14], M, 256, true};
-  if ((rc = gemm(ws + L.act[14], net->fc_w, net->fc_b, ws + L.act[15], 1, 1, M, 256, 512, 1, P, 0, stream))) return rc;
+  if ((rc = gemm(ws + L.act[14], net->fc_w, net->fc_b, ws + L.act[15], 1, 1, M, 256, 512, 1, P, pf, stream))) return rc;
   net->taps["lstm_o"] = Tap{ws + L.act[15], M, 512, true};
-  if ((rc = gemm(ws + L.act[15], net->head_w, net->head_b, ws + L.heads, 1, 1, M, 512, 64, 1, P, CTPN_F_OUT_F32, stream))) return rc;
+  if ((rc = gemm(ws + L.act[15], net->head_w, net->head_b, ws + L.heads, 1, 1, M, 512, 64, 1, P, CTPN_F_OUT_F32 | pf, stream))) return rc;
   const long long tot = (long long)M * 64;
   split_heads_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float *)(ws + L.heads), M, cls_score_out, bbox_pred_out);
   CTPN_LAUNCH_CHECK();

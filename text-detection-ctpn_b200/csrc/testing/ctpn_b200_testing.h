@@ -2,7 +2,7 @@
  * Test-only entry points of libctpn_b200_dbg.so (tests/_native/): float32 SIMT reference kernels with the product
  * kernels' contracts, and a hardware probe.  None of this is in the product library libctpn_b200.so or in
  * include/ctpn_b200.h.  The debug library is the product sources compiled with -DCTPN_DEBUG (ablation switches
- * CTPN_TC_DEBUG / CTPN_C1_DEBUG, tuning overrides CTPN_TC_BN / CTPN_TC_STAGES_* / CTPN_TC_MCAST, the "conv_simt" /
+ * CTPN_TC_DEBUG / CTPN_C1_DEBUG, tuning overrides CTPN_TC_BN / CTPN_TC_STAGES_* / CTPN_TC_MCAST / CTPN_TC_PROMOTE, the "conv_simt" /
  * "conv1_simt" options of ctpn_net_set_option) plus the two files in this directory.
  */
 #ifndef CTPN_B200_TESTING_H_
@@ -22,7 +22,7 @@ int ctpn_conv1_1(const void *src, int src_is_f32, const float *lut, const float 
 
 
 /* Same contract, float32 SIMT implementation (no tensor cores): kernel-level reference used
- * by the tests. */
+ * by the tests.  CTPN_F_PROMOTE is accepted and has no effect: these sums already round to nearest. */
 int ctpn_conv3x3_simt(const void *in_planes, const void *w_planes, const float *bias, void *out,
                       int B, int H, int W, int cin, int cout, int taps, int planes, int flags,
                       void *stream);

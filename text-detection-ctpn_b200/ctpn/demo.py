@@ -78,7 +78,7 @@ def main(argv=None):
     ap.add_argument("--weights", default=None,
                     help="TF checkpoint prefix / directory, frozen .pb, VGG .npy or .npz (default: cfg.TEST.checkpoints_path, "
                          "like demo.py:88-90)")
-    ap.add_argument("--planes", type=int, default=2, help="conv arithmetic: 1-3 bf16 planes, 4 = F16F8 (2 tensor-core units per MAC)")
+    ap.add_argument("--planes", type=int, default=2, help="conv arithmetic: 1-3 bf16 planes, 4 = F16F8 (2 tensor-core units per MAC), 5 = bf16x3 with promoted accumulation")
     ap.add_argument("--images", default=os.path.join(cfg.DATA_DIR, 'demo', '*'))
     ap.add_argument("--cfg", default=os.path.join(_PKG, 'ctpn', 'text.yml'))
     ap.add_argument("--native-connector", action="store_true",

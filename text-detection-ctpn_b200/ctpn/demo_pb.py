@@ -52,7 +52,8 @@ def detect_pb(sess, im_name):
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--pb", default="data/ctpn.pb")
-    ap.add_argument("--planes", type=int, default=2)
+    ap.add_argument("--planes", type=int, default=2,
+                    help="conv arithmetic: 1-3 bf16 planes, 4 = F16F8 (2 tensor-core units per MAC), 5 = bf16x3 with promoted accumulation")
     ap.add_argument("--images", default=None)
     ap.add_argument("--cfg", default=os.path.join(_PKG, 'ctpn', 'text.yml'))
     args = ap.parse_args(argv)

@@ -9,8 +9,11 @@ compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
 
 `planes` / `mode` select the arithmetic of the tensor-core layers (see include/ctpn_b200.h); accumulation is always
 float32:  1 / "bf16" = bf16 operands (1 unit per MAC);  2 / "bf16x2" = bf16x2 split, ~16 mantissa bits (3 units);
-3 / "bf16x3" = bf16x3 split, float32-equivalent products (6 units);  4 / "f16f8" = fp16 operands + e4m3 cross terms for the
-3x3 layers (2 units; head logits within 1e-3 of float32, 6-8e-4 measured; activation scales calibrated on the first batch).
+3 / "bf16x3" = bf16x3 split, exact float32 operands (6 units), but the tensor core's truncating accumulation leaves the
+head logits ~10x further from float64 than a float32 computation (DESIGN.md section 5);  5 / "bf16x3p" = bf16x3 with the
+main accumulator promoted to round-to-nearest float32 every 64 channels of a tap (CTPN_F_PROMOTE; 6 units);
+4 / "f16f8" = fp16 operands + e4m3 cross terms for the 3x3 layers (2 units; head logits within 1e-3 of float32, 6-8e-4
+measured; activation scales calibrated on the first batch).
 """
 import ctypes as C
 
@@ -27,7 +30,7 @@ DEFAULT_CFG = dict(RPN_PRE_NMS_TOP_N=12000, RPN_POST_NMS_TOP_N=1000, RPN_NMS_THR
 
 
 class Engine:
-    MODES = {"bf16": 1, "bf16x2": 2, "bf16x3": 3, "f16f8": 4}
+    MODES = {"bf16": 1, "bf16x2": 2, "bf16x3": 3, "f16f8": 4, "bf16x3p": 5}
 
     def __init__(self, weights=None, planes=2, device=0, cfg=None, conv_simt=False, keep_activations=False, streams=1, mode=None,
                  graph_max_batch=4):

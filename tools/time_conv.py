@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Perf experiment (test library: honours CTPN_TC_BN / CTPN_TC_STAGES_A / CTPN_TC_STAGES_B / CTPN_TC_MCAST / CTPN_TC_DEBUG):
-time one 3x3 layer of the conv stack alone, bf16 planes or F16F8.
+"""Perf experiment (test library: honours CTPN_TC_BN / CTPN_TC_STAGES_A / CTPN_TC_STAGES_B / CTPN_TC_MCAST / CTPN_TC_DEBUG /
+CTPN_TC_PROMOTE): time one 3x3 layer of the conv stack alone, bf16 planes, bf16x3 with promoted accumulation, or F16F8.
 
     CTPN_TC_STAGES_B=2 python tools/time_conv.py --B 32 --H 75 --W 112 --cin 512 --cout 512 --mode f16f8
+    CTPN_TC_PROMOTE=4 python tools/time_conv.py --B 32 --H 37 --W 56 --cin 512 --cout 512 --mode bf16x3p
 """
 import argparse
 import os
@@ -20,7 +21,8 @@ for k, d in dict(B=32, H=75, W=112, cin=512, cout=512, flags=1, reps=20).items()
 ap.add_argument("--mode", default="f16f8")
 a = ap.parse_args()
 dev = torch.device("cuda", 0)
-planes = {"bf16": 1, "bf16x2": 2, "bf16x3": 3, "f16f8": 2}[a.mode]
+planes = {"bf16": 1, "bf16x2": 2, "bf16x3": 3, "bf16x3p": 3, "f16f8": 2}[a.mode]
+flags = a.flags | (64 if a.mode == "bf16x3p" else 0)       # CTPN_F_PROMOTE (interval: CTPN_TC_PROMOTE)
 nin = a.B * a.H * a.W * a.cin
 x = torch.randint(0, 60, (planes * nin * 2,), dtype=torch.uint8, device=dev)            # small positive operand bytes
 w = torch.randint(0, 60, (planes * a.cout * 9 * a.cin * 2,), dtype=torch.uint8, device=dev)
@@ -34,7 +36,7 @@ def run():
     if a.mode == "f16f8":
         N.check(N.lib.ctpn_conv3x3_f16f8(N.ptr(x), N.ptr(w), N.ptr(b), N.ptr(out), a.B, a.H, a.W, a.cin, a.cout, 9, a.flags, 1.0, 1.0, 1.0, 1.0, N.stream_ptr()), "conv")
     else:
-        N.check(N.lib.ctpn_conv3x3(N.ptr(x), N.ptr(w), N.ptr(b), N.ptr(out), a.B, a.H, a.W, a.cin, a.cout, 9, planes, a.flags, N.stream_ptr()), "conv")
+        N.check(N.lib.ctpn_conv3x3(N.ptr(x), N.ptr(w), N.ptr(b), N.ptr(out), a.B, a.H, a.W, a.cin, a.cout, 9, planes, flags, N.stream_ptr()), "conv")
 
 
 for _ in range(3):
