@@ -21,8 +21,8 @@
 //     shuffles: the window of a pixel lives in lanes l, l^1, l^8, l^9) -> re-split into planes (cvt.rn.bf16x2.f32) ->
 //     transpose through swizzled shared memory -> 16-byte stores that cover one pixel's 64 contiguous bytes with 4 lanes
 //     (or float32 output).
-// 3x3 layers run as 2-CTA clusters that share every weight tile by TMA multicast (template parameter MC; CTPN_TC_MCAST=0
-// selects the single-CTA variant).
+// Small and promoted 3x3 layers run as 2-CTA clusters that share every weight tile by TMA multicast (template parameter MC;
+// CTPN_TC_MCAST=0 selects the single-CTA variant everywhere); large unpromoted ones run one CTA per SM (conv_tc_run).
 // Persistent CTAs (one per SM), warp-specialised: warp 0 weight (B) producer, warp 1 activation (A) producer,
 // warpgroups 1 and 2 MMAs + epilogue.  Reference: lib/networks/network.py:160-196.
 #include <cuda.h>
@@ -731,8 +731,14 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   if (planes > 1 && BN > 128) BN = 128;   // main + cross accumulators: 2 * BN / 2 registers per thread (F16F8 too)
   while (BN > cout || cout % BN) BN >>= 1;
   const long long m_tiles = (long long)B * p.tiles_x * p.tiles_y;
-  // weight-tile multicast over 2-CTA clusters (3x3 layers with at least one pair of pixel tiles per SM pair)
-  const bool mc = taps == 9 && tuning().mcast != 0 && m_tiles >= 2;
+  // Weight-tile multicast over 2-CTA clusters, for 3x3 layers with at least one pair of pixel tiles and, unpromoted, fewer
+  // than kMcMaxTilesPerSm output tiles per SM.  At batch scale the single-CTA kernel is about twice as fast: on one H100
+  // (400 W limit), batch 32 x 600x900 F16F8, conv1_2 6.5 against 14.0 ms, conv3_2 5.1 against 8.7 ms and conv4_2 4.5
+  // against 8.7 ms (tools/time_conv.py with CTPN_TC_MCAST=0).  Promoted layers keep multicast: their single-CTA kernel
+  // runs at BN = 64.
+  constexpr long long kMcMaxTilesPerSm = 16;
+  const bool mc = taps == 9 && tuning().mcast != 0 && m_tiles >= 2 &&
+                  (promote || m_tiles * (cout / BN) < kMcMaxTilesPerSm * g_sms[dev]);
   // promoted single-CTA 3x3 layers (a map of one 16 x 8 tile) run at BN = 64: with three accumulators that kernel
   // spills registers at BN = 128, the multicast and taps = 1 ones do not
   if (promote && taps == 9 && !mc && BN > 64) BN = 64;
