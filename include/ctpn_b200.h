@@ -93,6 +93,14 @@ int ctpn_proposals(const float *cls, int cls_is_logit, const float *bbox, const 
                    float nms_thresh, float min_size, int anchors_py2, float *rois_out,
                    int *index_out, int *count_out, void *workspace, size_t workspace_bytes,
                    void *stream);
+/* Ragged batch (see ctpn_net_forward_ragged): feat_hw (device int32 [batch][2]) is each image's feature-map size (fh, fw)
+ * within the H x W canvas of the head tensors.  Anchors of cells outside it are never valid and their head values are
+ * never read; index_out is image-local, (h * fw + w) * 10 + a.  Per image the result is that of ctpn_proposals on the image's
+ * own fh x fw heads.  Same workspace as ctpn_proposals for (batch, H, W). */
+int ctpn_proposals_ragged(const float *cls, int cls_is_logit, const float *bbox, const float *im_info, const int *feat_hw,
+                          int batch, int H, int W, int feat_stride, int pre_nms_topN, int post_nms_topN, float nms_thresh,
+                          float min_size, int anchors_py2, float *rois_out, int *index_out, int *count_out,
+                          void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- network stages --------------------------------------------------------------------
  * Activation format ("planes"): P in {1,2,3} bf16 tensors [P][B][H][W][C] whose element-wise
@@ -180,6 +188,15 @@ size_t ctpn_net_workspace_bytes(const ctpn_net_t *net, int B, int H, int W);
 int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_f32, int B, int H, int W,
                      float *cls_score_out, float *bbox_pred_out, void *workspace,
                      size_t workspace_bytes, void *stream);
+/* Ragged batch: B images of different sizes on one canvas [B][H][W][3]; image b occupies rows < h_b and columns < w_b of its
+ * slice (sizes: device int32 [B][2] = (h_b, w_b), 16 <= h_b <= H, 16 <= w_b <= W; a size beyond the canvas is clamped to it).
+ * The canvas outside an image is never read.  Every layer stores exact zeros outside the image's extent at its level,
+ * (h_b >> k, w_b >> k) after k pools, which the next 3x3 layer takes as its SAME padding; so each image's head tensors within
+ * (h_b >> 4, w_b >> 4) equal ctpn_net_forward of that image alone, bit for bit, in every arithmetic.  The head values outside
+ * that extent are unspecified.  Workspace: ctpn_net_workspace_bytes(net, B, H, W). */
+int ctpn_net_forward_ragged(ctpn_net_t *net, const void *images, int src_is_f32, const int *sizes, int B, int H, int W,
+                            float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes,
+                            void *stream);
 /* feature-map size after the four VALID pools */
 int ctpn_net_feature_hw(int H, int W, int *fh, int *fw);
 /* Debug tap: copies the most recent forward's named activation ("conv1_1" ... "rpn_conv/3x3",

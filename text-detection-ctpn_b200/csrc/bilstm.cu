@@ -10,6 +10,10 @@
 // direction, so Wh is read from shared memory once per RG rows.  All arithmetic is float32; the mat-vec keeps even-k and
 // odd-k partial sums (added at the end) so that one 16-byte weight load feeds two k.
 //
+// Ragged batches (sizes != null): row b * FH + y is a row of image b with (h_b >> 4, w_b >> 4) feature cells; it runs
+// w_b >> 4 steps when y < h_b >> 4 (none otherwise), the backward direction starting at its own last column, and its outputs
+// past that length are zero.  A cluster runs to the longest of its rows; each row's arithmetic is that of a uniform batch.
+//
 // TF 1.3 LSTMCell: gates (i, j, f, o) = [x, h] . kernel + bias;
 //   c = sigmoid(f + 1) * c + sigmoid(i) * tanh(j);  h = sigmoid(o) * tanh(c).
 #include <cooperative_groups.h>
@@ -39,7 +43,7 @@ template <bool FAST> __device__ __forceinline__ float lstm_tanh(float x) {
 template <int RG, int NC, bool FAST>
 __global__ void __launch_bounds__(256, NC == 4 ? 2 : 1)
 bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, const float *__restrict__ wh_bw,
-              __nv_bfloat16 *__restrict__ out, int R, int W, int planes) {
+              __nv_bfloat16 *__restrict__ out, int R, int W, int planes, const int *__restrict__ sizes, int FH) {
   constexpr int kUnits = kHid / NC;          // hidden units of this CTA
   constexpr int kLocalCols = 4 * kUnits;     // their i, j, f, o gate columns
   constexpr int kCG = kLocalCols / 4;        // column groups (4 adjacent columns per thread)
@@ -48,6 +52,7 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
   float *Ws = smem;                          // [128][kLocalCols]  recurrent weights of this CTA's units
   float *hbuf = Ws + kHid * kLocalCols;      // [2][RG][128] full hidden state, double buffered
   float *gates = hbuf + 2 * RG * kHid;       // [RG][256]    pre-activations of this CTA's columns
+  __shared__ int len[RG];                    // sequence length of each row of the group (0: no row / a dead row)
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   static_assert(NC == 2 || NC == 4, "cluster of 2 or 4 CTAs");
@@ -74,6 +79,15 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
         wh[k * kGates + (lc / kUnits) * kHid + rank * kUnits + (lc % kUnits)];
   }
   for (int i = t; i < 2 * RG * kHid; i += 256) hbuf[i] = 0.f;
+  if (t < RG) {
+    const int row = row0 + t;
+    int n = row < R ? W : 0;
+    if (sizes && row < R) {      // clamped to the canvas: a wrong size never addresses outside it
+      const int b = row / FH, y = row - b * FH;
+      n = y < min(FH, __ldg(sizes + 2 * b) >> 4) ? max(0, min(W, __ldg(sizes + 2 * b + 1) >> 4)) : 0;
+    }
+    len[t] = n;
+  }
   float *peer_h[NC];
 #pragma unroll
   for (int r = 0; r < NC; ++r) peer_h[r] = cluster.map_shared_rank(hbuf, r);
@@ -82,17 +96,18 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
 #pragma unroll
   for (int q = 0; q < kCellRows; ++q) c_state[q] = 0.f;
   cluster.sync();
+  int steps = 0;
+  for (int r = 0; r < RG; ++r) steps = max(steps, len[r]);
 
   const long long plane_stride = (long long)R * W * 2 * kHid;
   float4 xnext[RT];
 #pragma unroll
   for (int r = 0; r < RT; ++r) {
-    const int row = row0 + rg * RT + r;
-    xnext[r] = row < R ? __ldg(reinterpret_cast<const float4 *>(xproj + ((long long)row * W + (dir ? W - 1 : 0)) * (2 * kGates) + dir * kGates + gcol0))
-                       : make_float4(0.f, 0.f, 0.f, 0.f);
+    const int row = row0 + rg * RT + r, n = len[rg * RT + r];
+    xnext[r] = n > 0 ? __ldg(reinterpret_cast<const float4 *>(xproj + ((long long)row * W + (dir ? n - 1 : 0)) * (2 * kGates) + dir * kGates + gcol0))
+                     : make_float4(0.f, 0.f, 0.f, 0.f);
   }
-  for (int step = 0; step < W; ++step) {
-    const int tpos = dir ? W - 1 - step : step;
+  for (int step = 0; step < steps; ++step) {
     const float *hc = hbuf + (step & 1) * RG * kHid;
     const int hn_off = ((step + 1) & 1) * RG * kHid;
     // acc[r][c] = (sum over even k, sum over odd k) for local column lc0 + c: each ffma2_rn advances two k at once with the
@@ -104,12 +119,12 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
       acc[r][0] = make_float2(x.x, 0.f); acc[r][1] = make_float2(x.y, 0.f);
       acc[r][2] = make_float2(x.z, 0.f); acc[r][3] = make_float2(x.w, 0.f);
     }
-    if (step + 1 < W) {   // x-projection of the next step: in flight during this step's mat-vec
-      const int tn = dir ? W - 2 - step : step + 1;
+    if (step + 1 < steps) {   // x-projection of the next step: in flight during this step's mat-vec
 #pragma unroll
       for (int r = 0; r < RT; ++r) {
-        const int row = row0 + rg * RT + r;
-        if (row < R) xnext[r] = __ldg(reinterpret_cast<const float4 *>(xproj + ((long long)row * W + tn) * (2 * kGates) + dir * kGates + gcol0));
+        const int row = row0 + rg * RT + r, n = len[rg * RT + r];
+        const int tn = dir ? n - 2 - step : step + 1;
+        if (step + 1 < n) xnext[r] = __ldg(reinterpret_cast<const float4 *>(xproj + ((long long)row * W + tn) * (2 * kGates) + dir * kGates + gcol0));
       }
     }
     const float4 *w_lo = reinterpret_cast<const float4 *>(Ws) + cg;                       // columns lc0, lc0 + 1
@@ -149,21 +164,33 @@ bilstm_kernel(const float *__restrict__ xproj, const float *__restrict__ wh_fw, 
       const int u = rank * kUnits + ul;
 #pragma unroll
       for (int pr = 0; pr < NC; ++pr) peer_h[pr][hn_off + r * kHid + u] = h;     // own copy and every peer's (DSMEM)
-      const int row = row0 + r;
-      if (row < R) {
+      const int row = row0 + r, n = len[r];
+      if (row < R) {     // a row past its length writes a zero at column `step` instead (columns >= steps: below)
         __nv_bfloat16 pl[3];
-        split_planes(h, planes, pl);
+        split_planes(step < n ? h : 0.f, planes, pl);
+        const int tpos = step >= n ? step : dir ? n - 1 - step : step;
         const long long o = ((long long)row * W + tpos) * (2 * kHid) + dir * kHid + u;
         for (int p = 0; p < planes; ++p) out[p * plane_stride + o] = pl[p];
       }
     }
     cluster.sync();   // h_{t} of both halves visible in both CTAs; also orders the gates[] reuse
   }
+  // ragged batch: the columns past the group's longest row are zero
+  for (int step = steps; step < W; ++step) {
+#pragma unroll
+    for (int q = 0; q < kCellRows; ++q) {
+      const int row = row0 + (t / kUnits) + (256 / kUnits) * q;
+      if (row < R) {
+        const long long o = ((long long)row * W + step) * (2 * kHid) + dir * kHid + rank * kUnits + ul;
+        for (int p = 0; p < planes; ++p) out[p * plane_stride + o] = __float2bfloat16_rn(0.f);
+      }
+    }
+  }
 }
 
 template <int RG, int NC>
 static int launch_bilstm(const float *xproj, const float *wh_fw, const float *wh_bw, void *out, int R, int W, int planes,
-                         cudaStream_t st) {
+                         const int *sizes, int FH, cudaStream_t st) {
   constexpr int kLocalCols = 4 * kHid / NC;
   const size_t smem = (size_t)(kHid * kLocalCols + 2 * RG * kHid + RG * kLocalCols) * sizeof(float);
   auto kernel = planes <= 2 ? bilstm_kernel<RG, NC, true> : bilstm_kernel<RG, NC, false>;
@@ -180,7 +207,7 @@ static int launch_bilstm(const float *xproj, const float *wh_fw, const float *wh
   cfg.stream = st;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  CTPN_CUDA(cudaLaunchKernelEx(&cfg, kernel, xproj, wh_fw, wh_bw, (__nv_bfloat16 *)out, R, W, planes));
+  CTPN_CUDA(cudaLaunchKernelEx(&cfg, kernel, xproj, wh_fw, wh_bw, (__nv_bfloat16 *)out, R, W, planes, sizes, FH));
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
 }
@@ -191,8 +218,13 @@ using namespace ctpn;
 
 extern "C" int ctpn_bilstm_recurrent(const float *xproj, const float *wh_fw, const float *wh_bw, void *out_planes, int R,
                                      int W, int planes, void *stream) {
+  return bilstm_ragged(xproj, wh_fw, wh_bw, out_planes, R, W, planes, nullptr, R, stream);
+}
+
+int ctpn::bilstm_ragged(const float *xproj, const float *wh_fw, const float *wh_bw, void *out_planes, int R, int W, int planes,
+                        const int *sizes, int FH, void *stream) {
   CTPN_REQUIRE(xproj && wh_fw && wh_bw && out_planes, "ctpn_bilstm_recurrent: null pointer");
-  CTPN_REQUIRE(R > 0 && W > 0, "ctpn_bilstm_recurrent: bad shape R=%d W=%d", R, W);
+  CTPN_REQUIRE(R > 0 && W > 0 && FH > 0, "ctpn_bilstm_recurrent: bad shape R=%d W=%d", R, W);
   CTPN_REQUIRE(planes >= 1 && planes <= 3, "ctpn_bilstm_recurrent: planes must be 1..3");
   cudaStream_t st = (cudaStream_t)stream;
   // Rows per cluster (RG): the fewest that still run every cluster in ONE wave.  A CTA holds 130-210 KiB of shared memory,
@@ -208,11 +240,11 @@ extern "C" int ctpn_bilstm_recurrent(const float *xproj, const float *wh_fw, con
   auto fits = [&](int rg) { return (R + rg - 1) / rg <= per_wave; };
 #ifdef CTPN_DEBUG
   static const int force_nc = [] { const char *e = getenv("CTPN_LSTM_NC"); return e ? atoi(e) : 0; }();
-  if (!fits(16) && force_nc == 4) return launch_bilstm<32, 4>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (!fits(16) && force_nc == 4) return launch_bilstm<32, 4>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
 #endif
-  if (fits(4)) return launch_bilstm<4, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  if (fits(8)) return launch_bilstm<8, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  if (fits(16)) return launch_bilstm<16, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  if (fits(32)) return launch_bilstm<32, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
-  return launch_bilstm<40, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, st);
+  if (fits(4)) return launch_bilstm<4, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
+  if (fits(8)) return launch_bilstm<8, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
+  if (fits(16)) return launch_bilstm<16, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
+  if (fits(32)) return launch_bilstm<32, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
+  return launch_bilstm<40, 2>(xproj, wh_fw, wh_bw, out_planes, R, W, planes, sizes, FH, st);
 }

@@ -47,6 +47,21 @@ struct ProfScope {
   int idx_;
 };
 
+// ---- ragged batches (ctpn_net_forward_ragged) -----------------------------------------------
+// The network stages with per-image extents: sizes = device int32 [B][2] full-resolution image sizes (h, w) of a batch
+// whose canvas is [B][H][W]; a stage whose output is k pools down (shift = k) treats (h >> k, w >> k), clamped to its
+// frame, as the image and stores zeros outside it.  sizes = nullptr is the uniform batch (the public entry points).
+int conv1_1_tc_ragged(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias, void *out_planes,
+                      int B, int H, int W, int planes, bool outq, float out_s, float out_t, const int *sizes, void *stream);
+int conv3x3_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
+                   int cout, int taps, int planes, int flags, const int *sizes, int shift, void *stream);
+int conv3x3_f16f8_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
+                         int cout, int taps, int flags, float inv_main, float inv_cross, float out_s, float out_t,
+                         const int *sizes, int shift, void *stream);
+// R = B * rows_per_image rows; row b * rows_per_image + y runs (h_b >> 4, w_b >> 4) steps and is zero outside them
+int bilstm_ragged(const float *xproj, const float *wh_fw, const float *wh_bw, void *out_planes, int R, int W, int planes,
+                  const int *sizes, int rows_per_image, void *stream);
+
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 

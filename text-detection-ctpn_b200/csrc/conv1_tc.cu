@@ -42,7 +42,17 @@ struct Conv1TcParams {
   int debug;   // test library only (CTPN_C1_DEBUG bits): 1 skip patch staging, 2 skip tile build, 4 skip stores, 8 skip epilogue math
   long long plane_stride;
   float out_s, out_t, out_rs;    // OUTQ: F16F8 output quantisation (common.cuh), out_rs = 2^11 * out_t / out_s
+  const int *sizes;              // ragged batch: device int32 [B][2] image sizes (h, w); pixels outside are SAME padding
 };
+
+// extent of image b: its (h, w) from sizes clamped to the canvas, or the canvas
+__device__ __forceinline__ void c1_extent(const Conv1TcParams &p, int b, int &eh, int &ew) {
+  eh = p.H; ew = p.W;
+  if (p.sizes) {
+    eh = min(eh, __ldg(p.sizes + 2 * b));
+    ew = min(ew, __ldg(p.sizes + 2 * b + 1));
+  }
+}
 
 // OUTQ = 1: the output is written in the F16F8 activation format (fp16 plane + e4m3 value / residual plane) for a
 // conv1_2 that runs in the 2-unit arithmetic; the layer itself still multiplies P bf16 planes (K = 27: the MMAs are free).
@@ -117,12 +127,14 @@ conv1_tc_kernel(const Conv1TcParams p) {
       if (tile >= p.total_tiles) return;
       const unsigned b = (unsigned)tile / tpi, r = (unsigned)tile % tpi;
       const int y0 = (int)(r / tx) * 16, x0 = (int)(r % tx) * 8;
+      int eh, ew;
+      c1_extent(p, (int)b, eh, ew);
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         const int i = m + u * 128;
         const int xx = i % 10, yy = i / 10;
         const int gx = x0 + xx - 1, gy = y0 + yy - 1;
-        if (i < 180 && gx >= 0 && gx < p.W && gy >= 0 && gy < p.H && !C1_DBG(p, 1)) {
+        if (i < 180 && gx >= 0 && gx < ew && gy >= 0 && gy < eh && !C1_DBG(p, 1)) {
           const size_t off = (((size_t)b * p.H + gy) * p.W + gx) * 3;
           if (p.src_is_f32) {
             const float *q = reinterpret_cast<const float *>(p.src) + off;
@@ -143,7 +155,8 @@ conv1_tc_kernel(const Conv1TcParams p) {
       // two patches per group: a fast warp may stage tile n + 1 while a slow one still gathers from tile n's patch;
       // it cannot get to tile n + 2 before the group barrier of tile n + 1, which the slow warp reaches after tile n
       float *pt = patch + (grp * 2 + (n & 1)) * kC1tPatch;
-      // stage the 18 x 10 x 3 mean-subtracted input patch (zero outside the image: SAME padding of the blob)
+      // stage the 18 x 10 x 3 mean-subtracted input patch (zero outside the image: SAME padding of the blob; in a ragged batch
+      // the canvas outside the image's extent is never read)
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         const int i = m + u * 128;
@@ -210,6 +223,9 @@ conv1_tc_kernel(const Conv1TcParams p) {
       const unsigned b = (unsigned)tile / (unsigned)tiles_per_img, r = (unsigned)tile % (unsigned)tiles_per_img;
       const int y = (int)(r / (unsigned)p.tiles_x) * 16 + th, x = (int)(r % (unsigned)p.tiles_x) * 8 + tw;
       const bool ok = y < p.H && x < p.W;
+      int eh, ew;
+      c1_extent(p, (int)b, eh, ew);
+      const bool live = y < eh && x < ew;     // false: ragged padding, stored as zero (the bias row would make it ReLU(bias))
       const long long pix = ((long long)b * p.H + y) * p.W + x;
       const unsigned okmask = __ballot_sync(0xffffffffu, ok);
       long long spix[4];
@@ -260,6 +276,10 @@ conv1_tc_kernel(const Conv1TcParams p) {
         for (int q = 0; q < 8; ++q) {
           const float4 t = *reinterpret_cast<const float4 *>(epi + chunk * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
           v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+        }
+        if (!live) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = 0.f;
         }
         // the bias came in through the tensor core (k = 27 row of the weight tile x the builders' constant 1)
         if (OUTQ) {
@@ -346,8 +366,11 @@ static int launch_conv1_tc(Conv1TcParams &p, cudaStream_t st) {
   return CTPN_OK;
 }
 
-static int conv1_tc_run(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias,
-                        void *out_planes, int B, int H, int W, int planes, bool outq, float out_s, float out_t, void *stream) {
+}  // namespace ctpn
+
+int ctpn::conv1_1_tc_ragged(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias,
+                            void *out_planes, int B, int H, int W, int planes, bool outq, float out_s, float out_t,
+                            const int *sizes, void *stream) {
   CTPN_REQUIRE(src && w_hwio && bias && out_planes, "ctpn_conv1_1_tc: null pointer");
   CTPN_REQUIRE(src_is_f32 || lut, "ctpn_conv1_1_tc: uint8 input needs the mean-subtraction LUT");
   CTPN_REQUIRE(B > 0 && H > 0 && W > 0, "ctpn_conv1_1_tc: bad shape");
@@ -361,6 +384,7 @@ static int conv1_tc_run(const void *src, int src_is_f32, const float *lut, const
   p.total_tiles = (int)total;
   p.plane_stride = (long long)B * H * W * 64;
   p.out_s = p.out_t = p.out_rs = 1.f;
+  p.sizes = sizes;
   if (outq) {
     CTPN_REQUIRE(out_s > 0.f && out_t > 0.f, "ctpn_conv1_1_tc_f16f8: scales must be positive");
     p.out_s = out_s; p.out_t = out_t; p.out_rs = kResidualGain * out_t / out_s;
@@ -378,16 +402,14 @@ static int conv1_tc_run(const void *src, int src_is_f32, const float *lut, const
   return launch_conv1_tc<3>(p, st);
 }
 
-}  // namespace ctpn
-
 using namespace ctpn;
 
 extern "C" int ctpn_conv1_1_tc(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias,
                                void *out_planes, int B, int H, int W, int planes, void *stream) {
-  return conv1_tc_run(src, src_is_f32, lut, w_hwio, bias, out_planes, B, H, W, planes, false, 1.f, 1.f, stream);
+  return conv1_1_tc_ragged(src, src_is_f32, lut, w_hwio, bias, out_planes, B, H, W, planes, false, 1.f, 1.f, nullptr, stream);
 }
 
 extern "C" int ctpn_conv1_1_tc_f16f8(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias,
                                      void *out_planes, int B, int H, int W, float out_s, float out_t, void *stream) {
-  return conv1_tc_run(src, src_is_f32, lut, w_hwio, bias, out_planes, B, H, W, 2, true, out_s, out_t, stream);
+  return conv1_1_tc_ragged(src, src_is_f32, lut, w_hwio, bias, out_planes, B, H, W, 2, true, out_s, out_t, nullptr, stream);
 }

@@ -69,6 +69,11 @@ struct ConvTcParams {
   // zero rows keep the images' halos apart.  in_stack_h = rows per image incl. the pad row in the kernel's input frame (0 =
   // plain); out_rows = rows per image of the OUTPUT frame (Ho, or Ho + 1 when the output is stacked too).
   int in_stack_h, out_rows, out_stacked;
+  // Ragged batches (ctpn_net_forward_ragged): ext = device int32 [ext_n][2] full-resolution image sizes (h, w), or null.  An
+  // output pixel outside (h >> ext_shift, w >> ext_shift) of its image is stored as zero, so that the next 3x3 layer sees the
+  // zeros as SAME padding.  Masking is value-only: loads, MMAs and the multicast pairing do not change.
+  const int *ext;
+  int ext_shift, ext_n;
   double work;              // algorithmic FLOPs of the call (profiling label only)
   int stage_small;          // 1: 512-byte store-transpose block per epilogue warp (8 pixels per round)
   int promote_every;        // test library only (CTPN_TC_PROMOTE): pipeline steps per promoted main chain (product: 1)
@@ -350,6 +355,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           live = oy < p.in_stack_h - 1;
           if (!p.out_stacked) ok = ok && live;
         }
+      }
+      if (p.ext) {     // ragged batch: zero outside the image's extent at the output level (with a pool: the whole window)
+        const int ib = min(ob, p.ext_n - 1);
+        live = live && oy < (__ldg(p.ext + 2 * ib) >> p.ext_shift) && ox < (__ldg(p.ext + 2 * ib + 1) >> p.ext_shift);
       }
       const long long pix = ((long long)ob * p.out_rows + oy) * p.Wo + ox;
       // coalesced plane stores: the warp's 32-pixel x 32-channel block is transposed through shared memory so
@@ -658,7 +667,7 @@ namespace ctpn {
 struct QuantScales { float inv_main, inv_cross, out_s, out_t; };
 
 static int conv_tc_run(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
-                       int cout, int taps, int planes, int flags, const QuantScales *q, void *stream) {
+                       int cout, int taps, int planes, int flags, const QuantScales *q, const int *ext, int ext_shift, void *stream) {
   const bool f8 = q != nullptr, promote = (flags & CTPN_F_PROMOTE) != 0;
   CTPN_REQUIRE(!(promote && f8), "ctpn_conv3x3_f16f8: CTPN_F_PROMOTE is a flag of ctpn_conv3x3 with planes = 3");
   CTPN_REQUIRE(!promote || planes == 3, "ctpn_conv3x3: CTPN_F_PROMOTE needs planes = 3 (got %d)", planes);
@@ -716,6 +725,9 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   p.out_stacked = stack_out ? 1 : 0;
   p.out_plane_stride = (long long)img_B * p.out_rows * p.Wo * cout;
   p.cout_pad = cout;
+  p.ext = ext;
+  p.ext_shift = ext_shift;
+  p.ext_n = img_B;
   if (f8) {
     CTPN_REQUIRE(q->inv_main > 0.f && q->inv_cross > 0.f && q->out_s > 0.f && q->out_t > 0.f, "ctpn_conv3x3_f16f8: scales must be positive");
     p.inv_main = q->inv_main; p.inv_cross = q->inv_cross; p.out_s = q->out_s; p.out_t = q->out_t;
@@ -806,12 +818,25 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
 extern "C" int ctpn_conv3x3(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H,
                             int W, int cin, int cout, int taps, int planes, int flags, void *stream) {
   CTPN_REQUIRE(!(flags & CTPN_F_OUT_BF16X2), "ctpn_conv3x3: CTPN_F_OUT_BF16X2 is a flag of ctpn_conv3x3_f16f8");
-  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, planes, flags, nullptr, stream);
+  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, planes, flags, nullptr, nullptr, 0, stream);
 }
 
 extern "C" int ctpn_conv3x3_f16f8(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H,
                                   int W, int cin, int cout, int taps, int flags, float inv_main, float inv_cross, float out_s,
                                   float out_t, void *stream) {
   const QuantScales q{inv_main, inv_cross, out_s, out_t};
-  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, 2, flags, &q, stream);
+  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, 2, flags, &q, nullptr, 0, stream);
+}
+
+int ctpn::conv3x3_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
+                         int cout, int taps, int planes, int flags, const int *sizes, int shift, void *stream) {
+  CTPN_REQUIRE(!(flags & CTPN_F_OUT_BF16X2), "ctpn_conv3x3: CTPN_F_OUT_BF16X2 is a flag of ctpn_conv3x3_f16f8");
+  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, planes, flags, nullptr, sizes, shift, stream);
+}
+
+int ctpn::conv3x3_f16f8_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W,
+                               int cin, int cout, int taps, int flags, float inv_main, float inv_cross, float out_s, float out_t,
+                               const int *sizes, int shift, void *stream) {
+  const QuantScales q{inv_main, inv_cross, out_s, out_t};
+  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, 2, flags, &q, sizes, shift, stream);
 }

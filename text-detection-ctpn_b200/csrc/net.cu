@@ -282,22 +282,29 @@ __global__ void absmax_f16_kernel(const __half *__restrict__ x, long long n, uns
   if ((threadIdx.x & 31) == 0) atomicMax(out, bits);
 }
 
-// one 3x3 layer (or conv1_1 for l = 0) in the F16F8 arithmetic with the scales currently in the net
-static int run_layer_f16f8(ctpn_net *n, int l, const void *in, void *out, int B, int h, int w, bool stack, void *stream) {
+// pools before the output of layer l: a ragged batch's image of size (h, w) covers (h >> k, w >> k) of that output
+static int out_level(int l) {
+  int k = 0;
+  for (int i = 0; i <= l; ++i) k += kConvs[i].pool ? 1 : 0;
+  return k;
+}
+
+// one 3x3 layer in the F16F8 arithmetic with the scales currently in the net (sizes: ragged batch, or null)
+static int run_layer_f16f8(ctpn_net *n, int l, const void *in, void *out, int B, int h, int w, bool stack, const int *sizes, void *stream) {
   const ConvSpec &s = kConvs[l];
-  if (l == 0) return ctpn_conv1_1_tc_f16f8(in, 0, n->lut, n->c11_w, n->c11_b, out, B, h, w, n->act_s[0], n->act_t[0], stream);
   int flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0) | (l == 13 ? CTPN_F_OUT_BF16X2 : 0);   // rpn_conv feeds the bf16x2 matmuls
   if (stack && l >= 9 && l <= 12) flags |= CTPN_F_STACK_OUT;
   if (stack && l >= 10) flags |= CTPN_F_STACK_IN;
   const float inv_main = 1.f / (n->act_s[l - 1] * n->w_s[l]), inv_cross = 1.f / (kResidualGain * n->act_t[l - 1] * n->w_t[l]);
-  return ctpn_conv3x3_f16f8(in, n->conv_w[l], n->conv_b[l], out, B, h, w, s.cin, s.cout, 9, flags, inv_main, inv_cross,
-                            l == 13 ? 1.f : n->act_s[l], l == 13 ? 1.f : n->act_t[l], stream);
+  return conv3x3_f16f8_ragged(in, n->conv_w[l], n->conv_b[l], out, B, h, w, s.cin, s.cout, 9, flags, inv_main, inv_cross,
+                              l == 13 ? 1.f : n->act_s[l], l == 13 ? 1.f : n->act_t[l], sizes, out_level(l), stream);
 }
 
 // Activation scales from data: every layer is run with provisional scales, the maximum of its fp16 plane is read back,
 // the scales are fixed (fp16 plane below 2^14, e4m3 copy two binades below saturation) and the layer is run again so the
 // next one sees its final input.  Synchronises per layer; happens once (first forward, or after "recalibrate").
-static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, int B, int H, int W, const NetLayout &L, char *ws, void *stream) {
+static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, const int *sizes, int B, int H, int W, const NetLayout &L,
+                           char *ws, void *stream) {
   cudaStream_t st = (cudaStream_t)stream;
   int h = H, w = W;
   for (int l = 0; l < 13; ++l) {
@@ -307,8 +314,8 @@ static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, int 
     float s_try = 1.f;
     for (int attempt = 0; ; ++attempt) {
       n->act_s[l] = s_try; n->act_t[l] = 1.f;
-      int rc = l == 0 ? ctpn_conv1_1_tc_f16f8(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, s_try, 1.f, stream)
-                      : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, stream);
+      int rc = l == 0 ? conv1_1_tc_ragged(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, 2, true, s_try, 1.f, sizes, stream)
+                      : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, sizes, stream);
       if (rc) return rc;
       const long long cnt = (long long)B * (L.h[l] + ((L.stack && l >= 9 && l <= 12) ? 1 : 0)) * L.w[l] * kConvs[l].cout;
       CTPN_CUDA(cudaMemsetAsync(n->absmax_dev, 0, sizeof(unsigned), st));
@@ -331,8 +338,9 @@ static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, int 
       n->act_t[l] = exp2f(floorf(log2f(448.f / amax)) - 2.f);    // two binades of headroom; beyond that e4m3 saturates (cross term only)
       break;
     }
-    int rc = l == 0 ? ctpn_conv1_1_tc_f16f8(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, n->act_s[0], n->act_t[0], stream)
-                    : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, stream);
+    int rc = l == 0 ? conv1_1_tc_ragged(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, 2, true, n->act_s[0],
+                                        n->act_t[0], sizes, stream)
+                    : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, sizes, stream);
     if (rc) return rc;
     h = L.h[l]; w = L.w[l];
   }
@@ -392,11 +400,13 @@ extern "C" size_t ctpn_net_workspace_bytes(const ctpn_net_t *net, int B, int H, 
   return net_layout(net, B, H, W).total;
 }
 
-extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_f32, int B, int H, int W,
-                                float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes,
-                                void *stream) {
-  CTPN_REQUIRE(net && images && cls_score_out && bbox_pred_out && workspace, "ctpn_net_forward: null pointer");
-  CTPN_REQUIRE(B > 0 && H >= 16 && W >= 16, "ctpn_net_forward: bad shape B=%d H=%d W=%d", B, H, W);
+// The network forward of a uniform batch (sizes = null) or of a ragged one (sizes = device int32 [B][2] image sizes on the
+// canvas [B][H][W]): every stage gets the extents and stores zeros outside them, which the next 3x3 layer reads as padding.
+static int net_forward(ctpn_net *net, const void *images, int src_is_f32, const int *sizes, int B, int H, int W,
+                       float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes, void *stream) {
+#ifdef CTPN_DEBUG
+  CTPN_REQUIRE(!sizes || !(net->conv_simt || net->conv1_simt), "ctpn_net_forward_ragged: the SIMT reference kernels take uniform batches only");
+#endif
   int rc = finalize(net);
   if (rc) return rc;
   const NetLayout L = net_layout(net, B, H, W);
@@ -409,14 +419,15 @@ extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_
   net->taps.clear();
   if (net->f16f8) {
     // 2-unit arithmetic: conv1_1 and the thirteen 3x3 layers on F16F8 planes (calibrated on the first batch)
-    if (!net->calibrated && (rc = calibrate_f16f8(net, images, src_is_f32, B, H, W, L, ws, stream))) return rc;
+    if (!net->calibrated && (rc = calibrate_f16f8(net, images, src_is_f32, sizes, B, H, W, L, ws, stream))) return rc;
     int hh = H, ww = W;
-    if ((rc = ctpn_conv1_1_tc_f16f8(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, net->act_s[0], net->act_t[0], stream))) return rc;
+    if ((rc = conv1_1_tc_ragged(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, 2, true, net->act_s[0],
+                                net->act_t[0], sizes, stream))) return rc;
     net->taps["conv1_1"] = Tap{ws + L.act[0], (long long)B * H * W, 64, true, net->act_s[0], net->act_t[0]};
     for (int l = 1; l < 14; ++l) {
       if (L.stack && l == 9)      // conv4_3 writes only the image rows of its stacked output: the pad rows must be zero
         CTPN_CUDA(cudaMemsetAsync(ws + L.act[9], 0, (size_t)P * B * (L.h[9] + 1) * L.w[9] * kConvs[9].cout * 2, (cudaStream_t)stream));
-      if ((rc = run_layer_f16f8(net, l, ws + L.act[l - 1], ws + L.act[l], B, hh, ww, L.stack, stream))) return rc;
+      if ((rc = run_layer_f16f8(net, l, ws + L.act[l - 1], ws + L.act[l], B, hh, ww, L.stack, sizes, stream))) return rc;
       hh = L.h[l]; ww = L.w[l];
       const ConvSpec &s = kConvs[l];
       const bool stacked = L.stack && l >= 9 && l <= 12;
@@ -425,13 +436,21 @@ extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_
               stacked ? hh : 0, stacked ? ww : 0};
     }
   }
+  auto conv1 = [&](const void *src, int f32, const float *lut, const float *w, const float *b, void *out, int B_, int H_, int W_, int P_,
+                   void *st) {
 #ifdef CTPN_DEBUG
-  auto conv1 = (net->conv_simt || net->conv1_simt) ? ctpn_conv1_1 : ctpn_conv1_1_tc;
-  auto conv3 = net->conv_simt ? ctpn_conv3x3_simt : ctpn_conv3x3;
-#else
-  auto conv1 = ctpn_conv1_1_tc;
-  auto conv3 = ctpn_conv3x3;
+    if (net->conv_simt || net->conv1_simt) return ctpn_conv1_1(src, f32, lut, w, b, out, B_, H_, W_, P_, st);
 #endif
+    return conv1_1_tc_ragged(src, f32, lut, w, b, out, B_, H_, W_, P_, false, 1.f, 1.f, sizes, st);
+  };
+  // 3x3 layers pass the extents (output level `lvl`); the 1x1 matmuls run on the whole canvas (sizes = null)
+  auto conv3 = [&](const void *in, const void *w, const float *b, void *out, int B_, int H_, int W_, int cin, int cout, int taps, int P_,
+                   int flags, const int *sz, int lvl, void *st) {
+#ifdef CTPN_DEBUG
+    if (net->conv_simt) return ctpn_conv3x3_simt(in, w, b, out, B_, H_, W_, cin, cout, taps, P_, flags, st);
+#endif
+    return conv3x3_ragged(in, w, b, out, B_, H_, W_, cin, cout, taps, P_, flags, sz, lvl, st);
+  };
   const int pf = net->promote ? CTPN_F_PROMOTE : 0;     // CTPN_ARITH_BF16X3P: every conv_tc layer below
   if (!net->f16f8) {
   if ((rc = conv1(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, P, stream))) return rc;
@@ -445,25 +464,44 @@ extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_
     if (L.stack && l >= 10) flags |= CTPN_F_STACK_IN;
     if (L.stack && l == 9)      // conv4_3 writes only the image rows of its stacked output: the pad rows must be zero
       CTPN_CUDA(cudaMemsetAsync(ws + L.act[9], 0, (size_t)P * B * (L.h[9] + 1) * L.w[9] * kConvs[9].cout * 2, (cudaStream_t)stream));
-    if ((rc = conv3(ws + L.act[l - 1], net->conv_w[l], net->conv_b[l], ws + L.act[l], B, h, w, s.cin, s.cout, 9, P, flags, stream))) return rc;
+    if ((rc = conv3(ws + L.act[l - 1], net->conv_w[l], net->conv_b[l], ws + L.act[l], B, h, w, s.cin, s.cout, 9, P, flags, sizes,
+                    out_level(l), stream))) return rc;
     h = L.h[l]; w = L.w[l];
     net->taps[s.pool ? std::string(s.name) + "+pool" : std::string(s.name)] =
         Tap{ws + L.act[l], (long long)B * h * w, s.cout, true, 0.f, 0.f, stacked ? h : 0, stacked ? w : 0};
   }
   }
   const int M = B * L.fh * L.fw;
-  auto gemm = conv3;
-  if ((rc = gemm(ws + L.act[13], net->xproj_w, net->xproj_b, ws + L.xproj, 1, 1, M, 512, 1024, 1, P, CTPN_F_OUT_F32 | pf, stream))) return rc;
+  auto gemm = [&](const void *in, const void *w, const float *b, void *out, int cin, int cout, int flags) {
+    return conv3(in, w, b, out, 1, 1, M, cin, cout, 1, P, flags, nullptr, 0, stream);
+  };
+  if ((rc = gemm(ws + L.act[13], net->xproj_w, net->xproj_b, ws + L.xproj, 512, 1024, CTPN_F_OUT_F32 | pf))) return rc;
   net->taps["xproj"] = Tap{ws + L.xproj, M, 1024, false};
-  if ((rc = ctpn_bilstm_recurrent((const float *)(ws + L.xproj), net->wh_fw, net->wh_bw, ws + L.act[14], B * L.fh, L.fw, P, stream))) return rc;
+  if ((rc = bilstm_ragged((const float *)(ws + L.xproj), net->wh_fw, net->wh_bw, ws + L.act[14], B * L.fh, L.fw, P, sizes, L.fh, stream))) return rc;
   net->taps["lstm_out"] = Tap{ws + L.act[14], M, 256, true};
-  if ((rc = gemm(ws + L.act[14], net->fc_w, net->fc_b, ws + L.act[15], 1, 1, M, 256, 512, 1, P, pf, stream))) return rc;
+  if ((rc = gemm(ws + L.act[14], net->fc_w, net->fc_b, ws + L.act[15], 256, 512, pf))) return rc;
   net->taps["lstm_o"] = Tap{ws + L.act[15], M, 512, true};
-  if ((rc = gemm(ws + L.act[15], net->head_w, net->head_b, ws + L.heads, 1, 1, M, 512, 64, 1, P, CTPN_F_OUT_F32 | pf, stream))) return rc;
+  if ((rc = gemm(ws + L.act[15], net->head_w, net->head_b, ws + L.heads, 512, 64, CTPN_F_OUT_F32 | pf))) return rc;
   const long long tot = (long long)M * 64;
   split_heads_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float *)(ws + L.heads), M, cls_score_out, bbox_pred_out);
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
+}
+
+extern "C" int ctpn_net_forward(ctpn_net_t *net, const void *images, int src_is_f32, int B, int H, int W,
+                                float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes,
+                                void *stream) {
+  CTPN_REQUIRE(net && images && cls_score_out && bbox_pred_out && workspace, "ctpn_net_forward: null pointer");
+  CTPN_REQUIRE(B > 0 && H >= 16 && W >= 16, "ctpn_net_forward: bad shape B=%d H=%d W=%d", B, H, W);
+  return net_forward(net, images, src_is_f32, nullptr, B, H, W, cls_score_out, bbox_pred_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ctpn_net_forward_ragged(ctpn_net_t *net, const void *images, int src_is_f32, const int *sizes, int B, int H, int W,
+                                       float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes,
+                                       void *stream) {
+  CTPN_REQUIRE(net && images && sizes && cls_score_out && bbox_pred_out && workspace, "ctpn_net_forward_ragged: null pointer");
+  CTPN_REQUIRE(B > 0 && H >= 16 && W >= 16, "ctpn_net_forward_ragged: bad shape B=%d H=%d W=%d", B, H, W);
+  return net_forward(net, images, src_is_f32, sizes, B, H, W, cls_score_out, bbox_pred_out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int ctpn_net_debug_tap(ctpn_net_t *net, const char *name, float *out_f32, size_t capacity, size_t *count,

@@ -35,7 +35,8 @@ __global__ void __launch_bounds__(256)
 proposal_decode_kernel(const float *__restrict__ cls, int cls_is_logit, const float *__restrict__ bbox,
                        const float *__restrict__ im_info, int H, int W, int feat_stride, float min_size,
                        int py2, float nms_thresh, float4 *__restrict__ boxes, float *__restrict__ scores,
-                       uint32_t *__restrict__ keys, uint8_t *__restrict__ valid, int *__restrict__ unstructured) {
+                       uint32_t *__restrict__ keys, uint8_t *__restrict__ valid, int *__restrict__ unstructured,
+                       const int *__restrict__ feat_hw) {
   const int NA = H * W * 10;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int img = blockIdx.y;
@@ -44,6 +45,13 @@ proposal_decode_kernel(const float *__restrict__ cls, int cls_is_logit, const fl
   const int cell = i / 10;
   const int w = cell % W, h = cell / W;
   const size_t off = (size_t)img * NA + i;
+  if (feat_hw && (h >= feat_hw[2 * img] || w >= feat_hw[2 * img + 1])) {   // ragged batch: a cell outside the image's map
+    boxes[off] = make_float4(0.f, 0.f, 0.f, 0.f);
+    scores[off] = 0.f;
+    keys[off] = desc_key(0.f);
+    valid[off] = 0;
+    return;
+  }
   // fg score: channel 2a+1 of the pair (proposal_layer_tf.py:65)
   const float *cp = cls + ((size_t)img * H * W + cell) * 20 + 2 * a;
   float score;
@@ -201,7 +209,7 @@ __global__ void proposal_emit_kernel(const float4 *__restrict__ sorted_boxes, co
                                      const float *__restrict__ scores, const int *__restrict__ keep,
                                      const int *__restrict__ num, int NA, int max_n, int post, int kstride,
                                      float *__restrict__ rois, int *__restrict__ index_out,
-                                     int *__restrict__ count_out) {
+                                     int *__restrict__ count_out, int W, const int *__restrict__ feat_hw) {
   const int img = blockIdx.y;
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= post) return;
@@ -213,7 +221,14 @@ __global__ void proposal_emit_kernel(const float4 *__restrict__ sorted_boxes, co
     float4 b = sorted_boxes[(size_t)img * max_n + pos];
     r[0] = scores[(size_t)img * NA + idx];
     r[1] = b.x; r[2] = b.y; r[3] = b.z; r[4] = b.w;
-    if (index_out) index_out[(size_t)img * post + k] = idx;
+    if (index_out) {
+      int out_idx = idx;
+      if (feat_hw) {     // image-local (h * fw + w) * 10 + a: monotone in the canvas index, so the tie order is the same
+        const int cell = idx / 10;
+        out_idx = ((cell / W) * feat_hw[2 * img + 1] + cell % W) * 10 + idx % 10;
+      }
+      index_out[(size_t)img * post + k] = out_idx;
+    }
   } else {
     r[0] = r[1] = r[2] = r[3] = r[4] = 0.f;
     if (index_out) index_out[(size_t)img * post + k] = -1;
@@ -380,10 +395,10 @@ extern "C" size_t ctpn_proposals_workspace_bytes(int batch, int H, int W, int pr
   return proposal_layout(batch, NA, eff_max_n(NA, pre_nms_topN), eff_max_n(NA, pre_nms_topN)).total;
 }
 
-extern "C" int ctpn_proposals(const float *cls, int cls_is_logit, const float *bbox, const float *im_info, int batch,
-                              int H, int W, int feat_stride, int pre_nms_topN, int post_nms_topN, float nms_thresh,
-                              float min_size, int anchors_py2, float *rois_out, int *index_out, int *count_out,
-                              void *workspace, size_t workspace_bytes, void *stream) {
+static int proposals_run(const float *cls, int cls_is_logit, const float *bbox, const float *im_info, const int *feat_hw,
+                         int batch, int H, int W, int feat_stride, int pre_nms_topN, int post_nms_topN, float nms_thresh,
+                         float min_size, int anchors_py2, float *rois_out, int *index_out, int *count_out, void *workspace,
+                         size_t workspace_bytes, void *stream) {
   CTPN_REQUIRE(cls && bbox && im_info && rois_out && count_out, "ctpn_proposals: null pointer");
   CTPN_REQUIRE(batch > 0 && H > 0 && W > 0, "ctpn_proposals: bad shape batch=%d H=%d W=%d", batch, H, W);
   CTPN_REQUIRE(batch <= 65535, "ctpn_proposals: batch too large");
@@ -422,7 +437,7 @@ extern "C" int ctpn_proposals(const float *cls, int cls_is_logit, const float *b
   CTPN_CUDA(cudaMemsetAsync(unstructured, 0, (size_t)batch * sizeof(int), st));
   proposal_decode_kernel<<<g1, 256, 0, st>>>(cls, cls_is_logit, bbox, im_info, H, W, feat_stride, min_size,
                                              anchors_py2 ? 1 : 0, nms_thresh, boxes, scores, keys, valid,
-                                             try_columns ? unstructured : nullptr);
+                                             try_columns ? unstructured : nullptr, feat_hw);
   CTPN_LAUNCH_CHECK();
   CTPN_CUDA(cudaFuncSetAttribute(proposal_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSortSmem));
   // W <= 256: the sort kernel also buckets the survivors by column (one more 8-bit pass)
@@ -449,7 +464,24 @@ extern "C" int ctpn_proposals(const float *cls, int cls_is_logit, const float *b
   if (rc) return rc;
   dim3 g3(ceil_div(out_rows, 128), batch);
   proposal_emit_kernel<<<g3, 128, 0, st>>>(sorted_boxes, sorted_idx, scores, keep, num, NA, max_n, out_rows, post, rois_out,
-                                           index_out, count_out);
+                                           index_out, count_out, W, feat_hw);
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
+}
+
+extern "C" int ctpn_proposals(const float *cls, int cls_is_logit, const float *bbox, const float *im_info, int batch,
+                              int H, int W, int feat_stride, int pre_nms_topN, int post_nms_topN, float nms_thresh,
+                              float min_size, int anchors_py2, float *rois_out, int *index_out, int *count_out,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+  return proposals_run(cls, cls_is_logit, bbox, im_info, nullptr, batch, H, W, feat_stride, pre_nms_topN, post_nms_topN,
+                       nms_thresh, min_size, anchors_py2, rois_out, index_out, count_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int ctpn_proposals_ragged(const float *cls, int cls_is_logit, const float *bbox, const float *im_info,
+                                     const int *feat_hw, int batch, int H, int W, int feat_stride, int pre_nms_topN,
+                                     int post_nms_topN, float nms_thresh, float min_size, int anchors_py2, float *rois_out,
+                                     int *index_out, int *count_out, void *workspace, size_t workspace_bytes, void *stream) {
+  CTPN_REQUIRE(feat_hw, "ctpn_proposals_ragged: null feat_hw");
+  return proposals_run(cls, cls_is_logit, bbox, im_info, feat_hw, batch, H, W, feat_stride, pre_nms_topN, post_nms_topN,
+                       nms_thresh, min_size, anchors_py2, rois_out, index_out, count_out, workspace, workspace_bytes, stream);
 }

@@ -1,10 +1,12 @@
 """Command-line demo with the call structure of the reference's ctpn/demo.py:
 
-    python ctpn/demo.py [--weights CKPT_DIR|model.ckpt|ctpn.pb|W.npz] [--planes 2] [--images 'data/demo/*']
+    python ctpn/demo.py [--weights CKPT_DIR|model.ckpt|ctpn.pb|W.npz] [--planes 2] [--images 'data/demo/*'] [--batch N]
 
 ctpn(sess, net, image_name) keeps the reference signature (demo.py:55-68): read image, resize
 (short side 600, long side <= 1200), test_ctpn, TextDetector, write data/results/res_<stem>.txt
 and the annotated image.  `sess` is a ctpn_b200.Session (replaces tf.Session + Saver.restore).
+--batch N > 1 runs N images at a time through Engine.rois_ragged (images of different sizes in one batch), with the same
+resize, blob, TextDetector and output files per image (ctpn_batch).
 """
 from __future__ import print_function
 
@@ -24,7 +26,7 @@ sys.path.append(os.getcwd())
 
 from lib.networks.factory import get_network            # noqa: E402
 from lib.fast_rcnn.config import cfg, cfg_from_file     # noqa: E402
-from lib.fast_rcnn.test import test_ctpn                 # noqa: E402
+from lib.fast_rcnn.test import _get_image_blob, test_ctpn  # noqa: E402
 from lib.utils.timer import Timer                        # noqa: E402
 from lib.text_connector.detectors import TextDetector   # noqa: E402
 from lib.text_connector.text_connect_cfg import Config as TextLineCfg  # noqa: E402
@@ -73,6 +75,30 @@ def ctpn(sess, net, image_name):
     print(('Detection took {:.3f}s for {:d} object proposals').format(timer.total_time, boxes.shape[0]))
 
 
+def ctpn_batch(sess, image_names):
+    """ctpn() for several images at once: each is read, resized and turned into its blob as ctpn() / test_ctpn() do, the
+    blobs run as ragged batches (Engine.rois_ragged), and each result goes through TextDetector and draw_boxes."""
+    timer = Timer()
+    timer.tic()
+    imgs, scales, blobs, im_scales = [], [], [], []
+    for name in image_names:
+        img, scale = resize_im(cv2.imread(name), scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
+        blob, im_scale = _get_image_blob(img)
+        imgs.append(img)
+        scales.append(scale)
+        blobs.append(blob[0])
+        im_scales.append(float(im_scale[0]))
+    rois = sess.engine.rois_ragged(blobs, im_scales=im_scales)
+    for name, img, scale, r, im_scale in zip(image_names, imgs, scales, rois, im_scales):
+        scores, boxes = r[:, 0], r[:, 1:5] / np.float64(im_scale)      # the float64 division of test_ctpn
+        textdetector = TextDetector(native=NATIVE_CONNECTOR)
+        boxes = textdetector.detect(boxes, scores[:, np.newaxis], img.shape[:2])
+        draw_boxes(img, name, boxes, scale)
+        print('{:s}: {:d} text lines'.format(name, boxes.shape[0]))
+    timer.toc()
+    print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--weights", default=None,
@@ -83,6 +109,8 @@ def main(argv=None):
     ap.add_argument("--cfg", default=os.path.join(_PKG, 'ctpn', 'text.yml'))
     ap.add_argument("--native-connector", action="store_true",
                     help="build the text lines with the library's C++ connector (same lines, float32-rounding agreement)")
+    ap.add_argument("--batch", type=int, default=1,
+                    help="images per ragged batch (Engine.detect_ragged); 1 = one image at a time through test_ctpn")
     args = ap.parse_args(argv)
     global NATIVE_CONNECTOR
     NATIVE_CONNECTOR = args.native_connector
@@ -106,7 +134,13 @@ def main(argv=None):
         test_ctpn(sess, net, im)
     if args.planes == 4:                                # F16F8: take the activation scales from the first real image, not from the flat
         sess.engine.recalibrate()                       # grey warm-up image
-    for im_name in sorted(glob.glob(args.images)):
+    names = sorted(glob.glob(args.images))
+    if args.batch > 1:
+        for k in range(0, len(names), args.batch):
+            print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')
+            ctpn_batch(sess, names[k:k + args.batch])
+        return
+    for im_name in names:
         print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')
         print('Demo for {:s}'.format(im_name))
         ctpn(sess, net, im_name)

@@ -57,6 +57,7 @@ SIGNATURES = {
     "ctpn_nms_sorted": (_i, [_p, _p, _i, _i, _f, _i, _p, _p, _p, _z, _p]),
     "ctpn_proposals_workspace_bytes": (_z, [_i, _i, _i, _i]),
     "ctpn_proposals": (_i, [_p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _f, _f, _i, _p, _p, _p, _p, _z, _p]),
+    "ctpn_proposals_ragged": (_i, [_p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _f, _f, _i, _p, _p, _p, _p, _z, _p]),
     "ctpn_pack_weights": (_i, [_p, _i, _i, _i, _i, _i, _p, _p]),
     "ctpn_pack_weights_f16f8": (_i, [_p, _i, _i, _i, _i, _f, _f, _p, _p]),
     "ctpn_conv3x3_f16f8": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _f, _f, _f, _f, _p]),
@@ -70,6 +71,7 @@ SIGNATURES = {
     "ctpn_net_set_weight": (_i, [_p, C.c_char_p, _p, _z]),
     "ctpn_net_workspace_bytes": (_z, [_p, _i, _i, _i]),
     "ctpn_net_forward": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _p, _z, _p]),
+    "ctpn_net_forward_ragged": (_i, [_p, _p, _i, _p, _i, _i, _i, _p, _p, _p, _z, _p]),
     "ctpn_net_feature_hw": (_i, [_i, _i, C.POINTER(_i), C.POINTER(_i)]),
     "ctpn_net_debug_tap": (_i, [_p, C.c_char_p, _p, _z, C.POINTER(_z), _p]),
 }

@@ -6,6 +6,7 @@ compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
     eng = Engine(weights, planes=2)              # weights: {tf_variable_name: ndarray}
     scores, boxes = eng.detect(im)               # == lib.fast_rcnn.test.test_ctpn
     results = eng.detect_batch(uint8_batch)      # [B,H,W,3] -> list of (scores, boxes)
+    results = eng.detect_ragged([im0, im1, ...])  # images of different sizes, batched on shared canvases
 
 `planes` / `mode` select the arithmetic of the tensor-core layers (see include/ctpn_b200.h); accumulation is always
 float32:  1 / "bf16" = bf16 operands (1 unit per MAC);  2 / "bf16x2" = bf16x2 split, ~16 mantissa bits (3 units);
@@ -106,11 +107,23 @@ class Engine:
         N.check(N.lib.ctpn_net_feature_hw(H, W, C.byref(fh), C.byref(fw)), "ctpn_net_feature_hw")
         return fh.value, fw.value
 
+    def _sizes_device(self, sizes, B, H, W, least=16, what="sizes"):
+        """Per-image (h, w) of a ragged batch on its [B, H, W] canvas -> device int32 [B,2], checked on the host."""
+        s = sizes.cpu().numpy() if torch.is_tensor(sizes) else np.asarray(sizes)
+        s = np.asarray(s, np.int64).reshape(-1, 2) if s.size else s.reshape(0, 2)
+        if s.shape != (B, 2):
+            raise ValueError("%s: expected %d (h, w) pairs, got shape %s" % (what, B, tuple(np.shape(sizes))))
+        if (s[:, 0] > H).any() or (s[:, 1] > W).any() or (s < least).any():
+            raise ValueError("%s: every (h, w) must lie within the %dx%d canvas and be at least %d" % (what, H, W, least))
+        return torch.from_numpy(s.astype(np.int32)).to(self.device, non_blocking=False)
+
     # ---- stages ----------------------------------------------------------------------------
-    def forward_heads(self, images, ws_key="net"):
+    def forward_heads(self, images, ws_key="net", sizes=None):
         """images: CUDA tensor [B,H,W,3], uint8 BGR (mean subtraction fused) or float32 blob
         (already mean-subtracted, test.py:9).  Returns (rpn_cls_score [B,h,w,20] logits,
-        rpn_bbox_pred [B,h,w,40]) float32 CUDA tensors."""
+        rpn_bbox_pred [B,h,w,40]) float32 CUDA tensors.
+        sizes: [B,2] (h, w) per image for a ragged batch (image b in rows < h and columns < w of its canvas slice, the rest
+        ignored); each image's heads within (h >> 4, w >> 4) then equal a forward of that image alone.  None: uniform."""
         assert images.is_cuda and images.dim() == 4 and images.shape[3] == 3 and images.is_contiguous()
         is_f32 = images.dtype == torch.float32
         assert is_f32 or images.dtype == torch.uint8
@@ -120,8 +133,13 @@ class Engine:
         ws = self._workspace(ws_key, need)
         cls = torch.empty((B, fh, fw, 20), dtype=torch.float32, device=self.device)
         bbox = torch.empty((B, fh, fw, 40), dtype=torch.float32, device=self.device)
-        N.check(N.lib.ctpn_net_forward(self._net, N.ptr(images), int(is_f32), B, H, W, N.ptr(cls), N.ptr(bbox),
-                                       N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward")
+        if sizes is None:
+            N.check(N.lib.ctpn_net_forward(self._net, N.ptr(images), int(is_f32), B, H, W, N.ptr(cls), N.ptr(bbox),
+                                           N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward")
+        else:
+            sz = self._sizes_device(sizes, B, H, W)
+            N.check(N.lib.ctpn_net_forward_ragged(self._net, N.ptr(images), int(is_f32), N.ptr(sz), B, H, W, N.ptr(cls),
+                                                  N.ptr(bbox), N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward_ragged")
         return cls, bbox
 
     def recalibrate(self):
@@ -140,10 +158,12 @@ class Engine:
         N.check(N.lib.ctpn_net_debug_tap(self._net, name.encode(), N.ptr(out), out.numel(), C.byref(cnt), N.stream_ptr()), "debug_tap")
         return out
 
-    def proposals(self, cls, bbox, im_info, cls_is_logit=True, cfg=None, ws_key="prop", out=None):
+    def proposals(self, cls, bbox, im_info, cls_is_logit=True, cfg=None, ws_key="prop", out=None, feat_sizes=None):
         """Batched proposal layer (proposal_layer_tf.py:14-157) on CUDA tensors.
         Returns rois [B,post,5] (score,x1,y1,x2,y2), index [B,post] int32, count [B] int32.
-        out=(rois, count): write into these (contiguous) tensors instead of allocating."""
+        out=(rois, count): write into these (contiguous) tensors instead of allocating.
+        feat_sizes: [B,2] (fh, fw) per image of a ragged batch: only those cells of each image's heads are read, and index is
+        image-local ((h * fw + w) * 10 + a).  None: every cell."""
         c = dict(self.cfg)
         if cfg:
             c.update(cfg)
@@ -162,6 +182,13 @@ class Engine:
             count = torch.empty((B,), dtype=torch.int32, device=self.device)
         index = torch.empty((B, rows), dtype=torch.int32, device=self.device)
         im_info = im_info.to(device=self.device, dtype=torch.float32).contiguous()
+        if feat_sizes is not None:
+            fs = self._sizes_device(feat_sizes, B, H, W, least=1, what="feat_sizes")
+            N.check(N.lib.ctpn_proposals_ragged(N.ptr(cls.contiguous()), int(cls_is_logit), N.ptr(bbox.contiguous()), N.ptr(im_info),
+                                                N.ptr(fs), B, H, W, int(c["FEAT_STRIDE"]), pre, post, float(c["RPN_NMS_THRESH"]),
+                                                float(c["RPN_MIN_SIZE"]), int(bool(c["ANCHORS_PY2"])), N.ptr(rois), N.ptr(index),
+                                                N.ptr(count), N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_proposals_ragged")
+            return rois, index, count
         N.check(N.lib.ctpn_proposals(N.ptr(cls.contiguous()), int(cls_is_logit), N.ptr(bbox.contiguous()), N.ptr(im_info),
                                      B, H, W, int(c["FEAT_STRIDE"]), pre, post, float(c["RPN_NMS_THRESH"]),
                                      float(c["RPN_MIN_SIZE"]), int(bool(c["ANCHORS_PY2"])), N.ptr(rois), N.ptr(index),
@@ -185,18 +212,23 @@ class Engine:
         count = tail.view(torch.int32) if torch.is_tensor(tail) else tail.view(np.int32)
         return rois, count
 
-    def detect_packed(self, images, im_info, ws_tag=""):
+    def detect_packed(self, images, im_info, ws_tag="", sizes=None):
         """images: CUDA [B,H,W,3] uint8/float32; im_info: [B,3] tensor (blob_h, blob_w, scale).
         Returns ONE float32 device buffer [B*post*5 + B]: the rois of all images followed by the int32 counts
-        (bit pattern), so that the D2H / the multi-GPU gather of a batch's results is a single transfer."""
+        (bit pattern), so that the D2H / the multi-GPU gather of a batch's results is a single transfer.
+        sizes: [B,2] (h, w) per image of a ragged batch (see forward_heads), or None."""
         B = int(images.shape[0])
+        if sizes is not None:
+            sizes = np.asarray(sizes.cpu() if torch.is_tensor(sizes) else sizes, np.int64).reshape(-1, 2)
+            feat = sizes >> 4
         rows = self.result_rows()
         packed = torch.empty(B * rows * 5 + B, dtype=torch.float32, device=self.device)
         rois, count = self.unpack(packed, B, rows)
         n = min(self.streams, B)
         if n <= 1:
-            cls, bbox = self.forward_heads(images, ws_key="net" + ws_tag)
-            self.proposals(cls, bbox, im_info, cls_is_logit=True, ws_key="prop" + ws_tag, out=(rois, count))
+            cls, bbox = self.forward_heads(images, ws_key="net" + ws_tag, sizes=sizes)
+            self.proposals(cls, bbox, im_info, cls_is_logit=True, ws_key="prop" + ws_tag, out=(rois, count),
+                           feat_sizes=None if sizes is None else feat)
             return packed
         # sub-batches on side streams: the SIMT kernels of one sub-batch (conv1_1, BiLSTM, sort, NMS) run beside
         # the tensor-core kernels of the other (a persistent conv CTA leaves room for them on every SM)
@@ -210,8 +242,9 @@ class Engine:
             st.wait_stream(main)
             with torch.cuda.stream(st):
                 lo, hi = bounds[i], bounds[i + 1]
-                cls, bbox = self.forward_heads(images[lo:hi], ws_key="net%d" % i)
-                self.proposals(cls, bbox, im_info[lo:hi], cls_is_logit=True, ws_key="prop%d" % i, out=(rois[lo:hi], count[lo:hi]))
+                cls, bbox = self.forward_heads(images[lo:hi], ws_key="net%d" % i, sizes=None if sizes is None else sizes[lo:hi])
+                self.proposals(cls, bbox, im_info[lo:hi], cls_is_logit=True, ws_key="prop%d" % i, out=(rois[lo:hi], count[lo:hi]),
+                               feat_sizes=None if sizes is None else feat[lo:hi])
         for st in self._side[:n]:
             main.wait_stream(st)
         return packed
@@ -468,6 +501,56 @@ class Engine:
                     out[i] = r
         return out
 
+    def detect_ragged(self, images, im_scales=None, max_batch=32):
+        """Images of different sizes in shared batches: a list of HxWx3 uint8 BGR images or float32 mean-subtracted blobs
+        (H, W >= 16), with im_scales[i] the scale that made image i (default 1).  ragged_plan() groups them into batches of
+        at most `max_batch` on a canvas of each batch's largest H and W; every image is computed as if it ran alone
+        (ctpn_net_forward_ragged), with im_info (h, w, im_scale) of its own.  Returns [(scores, boxes / im_scale)] in input
+        order, as detect_batch returns them.  Raises ValueError on a bad image or scale list."""
+        scales = [1.0] * len(images) if im_scales is None else list(im_scales)
+        rois = self.rois_ragged(images, im_scales, max_batch)
+        return [(r[:, 0], r[:, 1:5] / np.float32(s)) for r, s in zip(rois, scales)]
+
+    def rois_ragged(self, images, im_scales=None, max_batch=32):
+        """detect_ragged's rois: one float32 [n,5] array (score, x1, y1, x2, y2) in blob coordinates per image, in input
+        order (test_ctpn divides these by its float64 im_scale; detect_batch by float32)."""
+        images = list(images)
+        n = len(images)
+        scales = [1.0] * n if im_scales is None else [float(s) for s in im_scales]
+        if len(scales) != n:
+            raise ValueError("detect_ragged: %d images but %d scales" % (n, len(scales)))
+        arrs, shapes, dtypes = [], [], []
+        for i, im in enumerate(images):
+            a = im.numpy() if torch.is_tensor(im) else np.asarray(im)
+            if a.ndim != 3 or a.shape[2] != 3 or a.dtype not in (np.uint8, np.float32):
+                raise ValueError("detect_ragged: image %d must be HxWx3 uint8 or float32 (got %s %s)" % (i, a.shape, a.dtype))
+            if a.shape[0] < 16 or a.shape[1] < 16:
+                raise ValueError("detect_ragged: image %d is %dx%d; both sides must be at least 16" % (i, a.shape[0], a.shape[1]))
+            arrs.append(a)
+            shapes.append((int(a.shape[0]), int(a.shape[1])))
+            dtypes.append(a.dtype.str)
+        out = [None] * n
+        rows = self.result_rows()
+        for idxs, (H, W) in ragged_plan(shapes, dtypes, max_batch):
+            B = len(idxs)
+            dt = torch.uint8 if arrs[idxs[0]].dtype == np.uint8 else torch.float32
+            canvas = self._pin("ragged", (B, H, W, 3), dt)        # padding keeps whatever it held: the kernels never read it
+            cn = canvas.numpy()
+            for k, i in enumerate(idxs):
+                h, w = shapes[i]
+                cn[k, :h, :w] = arrs[i]
+            info_h = self._pin("info", (B, 3), torch.float32)
+            info_h.numpy()[...] = [[shapes[i][0], shapes[i][1], scales[i]] for i in idxs]
+            sizes = np.array([shapes[i] for i in idxs], np.int64)
+            packed = self.detect_packed(canvas.to(self.device, non_blocking=True), info_h.to(self.device, non_blocking=True),
+                                        sizes=sizes)
+            out_h = self._pin("out", tuple(packed.shape), torch.float32)
+            out_h.copy_(packed, non_blocking=True)
+            torch.cuda.current_stream().synchronize()              # also frees the pinned canvas for the next batch
+            for i, r in zip(idxs, self._split_results(out_h, B, rows)):
+                out[i] = r
+        return out
+
     def resize_images(self, images, fx, fy=None):
         """cv2.resize(im, None, None, fx=fx, fy=fy, interpolation=cv2.INTER_LINEAR) of a uint8 batch [B,H,W,C] on the
         device (bit-exact with OpenCV; resize_im of ctpn/demo.py:21-25).  images: ndarray or torch tensor (host or
@@ -536,6 +619,28 @@ class Engine:
     def detect(self, image, im_scale=1.0):
         """Single image [H,W,3] -> (scores, boxes); the test_ctpn() contract."""
         return self.detect_batch(image[None], im_scale)[0]
+
+
+def ragged_plan(shapes, dtypes, max_batch=32):
+    """Batches of a ragged detect (Engine.detect_ragged): shapes [(H, W)], dtypes [str] of n images -> a list of
+    (indices, (canvas_H, canvas_W)).  Images are grouped by dtype and orientation (H > W or not), sorted by (H, W) within a
+    group, and each group is cut into chunks of at most max_batch; a chunk's canvas is its largest H and largest W.  Every
+    index appears in exactly one chunk."""
+    max_batch = int(max_batch)
+    if max_batch < 1:
+        raise ValueError("ragged_plan: max_batch must be >= 1")
+    if len(shapes) != len(dtypes):
+        raise ValueError("ragged_plan: %d shapes but %d dtypes" % (len(shapes), len(dtypes)))
+    groups = {}
+    for i, ((h, w), dt) in enumerate(zip(shapes, dtypes)):
+        groups.setdefault((str(dt), int(h) > int(w)), []).append(i)
+    plan = []
+    for key in sorted(groups):
+        idxs = sorted(groups[key], key=lambda i: (int(shapes[i][0]), int(shapes[i][1]), i))
+        for k in range(0, len(idxs), max_batch):
+            part = idxs[k:k + max_batch]
+            plan.append((part, (max(int(shapes[i][0]) for i in part), max(int(shapes[i][1]) for i in part))))
+    return plan
 
 
 # the 38 variables of the VGGnet_test graph (SURVEY.md App. A.2); a TF checkpoint also holds optimizer slots etc.
