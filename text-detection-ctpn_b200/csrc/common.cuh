@@ -53,11 +53,10 @@ struct ProfScope {
 // frame, as the image and stores zeros outside it.  sizes = nullptr is the uniform batch (the public entry points).
 int conv1_1_tc_ragged(const void *src, int src_is_f32, const float *lut, const float *w_hwio, const float *bias, void *out_planes,
                       int B, int H, int W, int planes, bool outq, float out_s, float out_t, const int *sizes, void *stream);
-int conv3x3_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
-                   int cout, int taps, int planes, int flags, const int *sizes, int shift, void *stream);
-int conv3x3_f16f8_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
-                         int cout, int taps, int flags, float inv_main, float inv_cross, float out_s, float out_t,
-                         const int *sizes, int shift, void *stream);
+// ctpn_conv3x3 (q = null) and ctpn_conv3x3_f16f8 (q = its scales, planes = 2) with the extents above (ext = sizes, ext_shift = shift)
+struct QuantScales { float inv_main, inv_cross, out_s, out_t; };
+int conv_tc_run(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
+                int cout, int taps, int planes, int flags, const QuantScales *q, const int *ext, int ext_shift, void *stream);
 // R = B * rows_per_image rows; row b * rows_per_image + y runs (h_b >> 4, w_b >> 4) steps and is zero outside them
 int bilstm_ragged(const float *xproj, const float *wh_fw, const float *wh_bw, void *out_planes, int R, int W, int planes,
                   const int *sizes, int rows_per_image, void *stream);

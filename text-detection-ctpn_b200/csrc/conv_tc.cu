@@ -659,16 +659,10 @@ static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, Conv
   return CTPN_OK;
 }
 
-}  // namespace ctpn
-
-using namespace ctpn;
-
-namespace ctpn {
-struct QuantScales { float inv_main, inv_cross, out_s, out_t; };
-
-static int conv_tc_run(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
-                       int cout, int taps, int planes, int flags, const QuantScales *q, const int *ext, int ext_shift, void *stream) {
+int conv_tc_run(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
+                int cout, int taps, int planes, int flags, const QuantScales *q, const int *ext, int ext_shift, void *stream) {
   const bool f8 = q != nullptr, promote = (flags & CTPN_F_PROMOTE) != 0;
+  CTPN_REQUIRE(f8 || !(flags & CTPN_F_OUT_BF16X2), "ctpn_conv3x3: CTPN_F_OUT_BF16X2 is a flag of ctpn_conv3x3_f16f8");
   CTPN_REQUIRE(!(promote && f8), "ctpn_conv3x3_f16f8: CTPN_F_PROMOTE is a flag of ctpn_conv3x3 with planes = 3");
   CTPN_REQUIRE(!promote || planes == 3, "ctpn_conv3x3: CTPN_F_PROMOTE needs planes = 3 (got %d)", planes);
   CTPN_REQUIRE(in_planes && w_planes && bias && out, "ctpn_conv3x3: null pointer");
@@ -813,11 +807,13 @@ static int conv_tc_run(const void *in_planes, const void *w_planes, const float 
   set_error("ctpn_conv3x3: no kernel for BN=%d planes=%d taps=%d", BN, planes, taps);
   return CTPN_ERR_INVALID;
 }
+
 }  // namespace ctpn
+
+using namespace ctpn;
 
 extern "C" int ctpn_conv3x3(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H,
                             int W, int cin, int cout, int taps, int planes, int flags, void *stream) {
-  CTPN_REQUIRE(!(flags & CTPN_F_OUT_BF16X2), "ctpn_conv3x3: CTPN_F_OUT_BF16X2 is a flag of ctpn_conv3x3_f16f8");
   return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, planes, flags, nullptr, nullptr, 0, stream);
 }
 
@@ -826,17 +822,4 @@ extern "C" int ctpn_conv3x3_f16f8(const void *in_planes, const void *w_planes, c
                                   float out_t, void *stream) {
   const QuantScales q{inv_main, inv_cross, out_s, out_t};
   return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, 2, flags, &q, nullptr, 0, stream);
-}
-
-int ctpn::conv3x3_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W, int cin,
-                         int cout, int taps, int planes, int flags, const int *sizes, int shift, void *stream) {
-  CTPN_REQUIRE(!(flags & CTPN_F_OUT_BF16X2), "ctpn_conv3x3: CTPN_F_OUT_BF16X2 is a flag of ctpn_conv3x3_f16f8");
-  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, planes, flags, nullptr, sizes, shift, stream);
-}
-
-int ctpn::conv3x3_f16f8_ragged(const void *in_planes, const void *w_planes, const float *bias, void *out, int B, int H, int W,
-                               int cin, int cout, int taps, int flags, float inv_main, float inv_cross, float out_s, float out_t,
-                               const int *sizes, int shift, void *stream) {
-  const QuantScales q{inv_main, inv_cross, out_s, out_t};
-  return conv_tc_run(in_planes, w_planes, bias, out, B, H, W, cin, cout, taps, 2, flags, &q, sizes, shift, stream);
 }

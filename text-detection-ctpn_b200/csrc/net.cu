@@ -45,7 +45,7 @@ struct ctpn_net {
   bool promote = false;     // CTPN_ARITH_BF16X3P: planes = 3 with CTPN_F_PROMOTE on every conv_tc layer
   float w_s[14] = {0}, w_t[14] = {0}, act_s[14] = {0}, act_t[14] = {0}, act_max[14] = {0};
   unsigned *absmax_dev = nullptr;
-  int conv_simt = 0, conv1_simt = 0, keep = 0;
+  int conv_simt = 0, keep = 0;
   std::map<std::string, std::vector<float>> host;
   bool dirty = true;
   std::vector<void *> owned;
@@ -187,42 +187,66 @@ static int finalize(ctpn_net *n) {
   return CTPN_OK;
 }
 
+// One conv layer of the net for a given batch shape, in the net's arithmetic
+struct ConvLayer {
+  size_t in, out;       // workspace offsets of the input and the output (conv1_1 reads the images, not `in`)
+  int h, w, ho, wo;     // input and output size
+  int flags;            // conv_tc flags of the 3x3 layers (conv1_1: 0)
+  int shift;            // pools up to the output: a ragged batch's image of size (h, w) covers (h >> shift, w >> shift) of it
+  bool stacked;         // output row-stacked as [B][ho + 1][wo]
+  long long elems;      // elements of one output plane as stored, pad rows included
+};
+
 struct NetLayout {
   bool stack;           // conv4_3's pooled output and conv5_1..conv5_3 outputs are row-stacked ([B][h + 1][w], zero pad rows)
-  size_t act[16];       // offsets of the 14 conv outputs + lstm_out + fc_out
-  size_t xproj, heads, total;
-  int h[15], w[15];     // spatial size of each conv output
+  ConvLayer conv[14];
+  size_t lstm, fc, xproj, heads, total;
   int fh, fw;
 };
 
 static NetLayout net_layout(const ctpn_net *n, int B, int H, int W) {
   NetLayout L;
   const int P = n->planes;
-  size_t sizes[16];
-  int h = H, w = W;
+  int h = H, w = W, shift = 0;
   for (int l = 0; l < 14; ++l) {
-    if (kConvs[l].pool) { h /= 2; w /= 2; }
-    L.h[l] = h; L.w[l] = w;
-    sizes[l] = (size_t)P * B * h * w * kConvs[l].cout * 2;
+    ConvLayer &c = L.conv[l];
+    c.h = h; c.w = w;
+    if (kConvs[l].pool) { h /= 2; w /= 2; ++shift; }
+    c.ho = h; c.wo = w; c.shift = shift;
   }
   L.fh = h; L.fw = w;
   // stack the 1/16-scale maps when one tall image needs fewer 16-row tiles than B separate ones (37 rows: 76 vs 96 at B = 32)
   L.stack = !n->conv_simt && ((long long)B * (h + 1) + 15) / 16 < (long long)B * ((h + 15) / 16);   // (the SIMT reference kernels of the test library know no stacking)
-  if (L.stack)
-    for (int l = 9; l <= 12; ++l) sizes[l] = (size_t)P * B * (h + 1) * w * kConvs[l].cout * 2;
+  size_t sizes[16];
+  for (int l = 0; l < 14; ++l) {
+    const ConvSpec &s = kConvs[l];
+    ConvLayer &c = L.conv[l];
+    c.stacked = L.stack && l >= 9 && l <= 12;
+    c.flags = 0;
+    if (l > 0) {
+      c.flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0) | (n->promote ? CTPN_F_PROMOTE : 0);
+      if (n->f16f8 && l == 13) c.flags |= CTPN_F_OUT_BF16X2;    // rpn_conv feeds the bf16x2 matmuls
+      if (c.stacked) c.flags |= CTPN_F_STACK_OUT;
+      if (L.stack && l >= 10) c.flags |= CTPN_F_STACK_IN;
+    }
+    c.elems = (long long)B * (c.ho + (c.stacked ? 1 : 0)) * c.wo * s.cout;
+    sizes[l] = (size_t)P * c.elems * 2;
+  }
   const size_t M = (size_t)B * h * w;
   sizes[14] = (size_t)P * M * 256 * 2;   // lstm_out
   sizes[15] = (size_t)P * M * 512 * 2;   // lstm_o (FC)
-  size_t o = 0;
+  size_t act[16], o = 0;
   if (n->keep) {
-    for (int i = 0; i < 16; ++i) { L.act[i] = o; o = align_up(o + sizes[i], 1024); }
+    for (int i = 0; i < 16; ++i) { act[i] = o; o = align_up(o + sizes[i], 1024); }
   } else {   // ping-pong between two buffers
     size_t even = 0, odd = 0;
     for (int i = 0; i < 16; ++i) (i & 1 ? odd : even) = std::max(i & 1 ? odd : even, sizes[i]);
     even = align_up(even, 1024); odd = align_up(odd, 1024);
-    for (int i = 0; i < 16; ++i) L.act[i] = (i & 1) ? even : 0;
+    for (int i = 0; i < 16; ++i) act[i] = (i & 1) ? even : 0;
     o = even + odd;
   }
+  for (int l = 0; l < 14; ++l) { L.conv[l].in = l ? act[l - 1] : 0; L.conv[l].out = act[l]; }
+  L.lstm = act[14]; L.fc = act[15];
   L.xproj = o; o = align_up(o + M * 1024 * sizeof(float), 1024);
   L.heads = o; o = align_up(o + M * 64 * sizeof(float), 1024);
   L.total = o;
@@ -282,44 +306,44 @@ __global__ void absmax_f16_kernel(const __half *__restrict__ x, long long n, uns
   if ((threadIdx.x & 31) == 0) atomicMax(out, bits);
 }
 
-// pools before the output of layer l: a ragged batch's image of size (h, w) covers (h >> k, w >> k) of that output
-static int out_level(int l) {
-  int k = 0;
-  for (int i = 0; i <= l; ++i) k += kConvs[i].pool ? 1 : 0;
-  return k;
-}
-
-// one 3x3 layer in the F16F8 arithmetic with the scales currently in the net (sizes: ragged batch, or null)
-static int run_layer_f16f8(ctpn_net *n, int l, const void *in, void *out, int B, int h, int w, bool stack, const int *sizes, void *stream) {
+// Layer l of the net in its arithmetic (sizes: ragged batch, or null).  (out_s, out_t) quantise an F16F8 output; other
+// modes and rpn_conv's bf16x2 output ignore them.  The input scales of an F16F8 layer are layer l - 1's in the net.
+static int run_conv(ctpn_net *n, const NetLayout &L, int l, const void *images, int src_is_f32, const int *sizes, int B,
+                    char *ws, float out_s, float out_t, void *stream) {
   const ConvSpec &s = kConvs[l];
-  int flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0) | (l == 13 ? CTPN_F_OUT_BF16X2 : 0);   // rpn_conv feeds the bf16x2 matmuls
-  if (stack && l >= 9 && l <= 12) flags |= CTPN_F_STACK_OUT;
-  if (stack && l >= 10) flags |= CTPN_F_STACK_IN;
-  const float inv_main = 1.f / (n->act_s[l - 1] * n->w_s[l]), inv_cross = 1.f / (kResidualGain * n->act_t[l - 1] * n->w_t[l]);
-  return conv3x3_f16f8_ragged(in, n->conv_w[l], n->conv_b[l], out, B, h, w, s.cin, s.cout, 9, flags, inv_main, inv_cross,
-                              l == 13 ? 1.f : n->act_s[l], l == 13 ? 1.f : n->act_t[l], sizes, out_level(l), stream);
+  const ConvLayer &c = L.conv[l];
+  if (!n->f16f8 || (c.flags & CTPN_F_OUT_BF16X2)) out_s = out_t = 1.f;
+  if (c.stacked && !(c.flags & CTPN_F_STACK_IN))    // a stacked output from an unstacked input: only the image rows are written
+    CTPN_CUDA(cudaMemsetAsync(ws + c.out, 0, (size_t)n->planes * c.elems * 2, (cudaStream_t)stream));
+#ifdef CTPN_DEBUG
+  if (n->conv_simt)
+    return l == 0 ? ctpn_conv1_1(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + c.out, B, c.h, c.w, n->planes, stream)
+                  : ctpn_conv3x3_simt(ws + c.in, n->conv_w[l], n->conv_b[l], ws + c.out, B, c.h, c.w, s.cin, s.cout, 9, n->planes,
+                                      c.flags, stream);
+#endif
+  if (l == 0)
+    return conv1_1_tc_ragged(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + c.out, B, c.h, c.w, n->planes, n->f16f8, out_s,
+                             out_t, sizes, stream);
+  QuantScales q{};
+  if (n->f16f8) q = {1.f / (n->act_s[l - 1] * n->w_s[l]), 1.f / (kResidualGain * n->act_t[l - 1] * n->w_t[l]), out_s, out_t};
+  return conv_tc_run(ws + c.in, n->conv_w[l], n->conv_b[l], ws + c.out, B, c.h, c.w, s.cin, s.cout, 9, n->planes, c.flags,
+                     n->f16f8 ? &q : nullptr, sizes, c.shift, stream);
 }
 
 // Activation scales from data: every layer is run with provisional scales, the maximum of its fp16 plane is read back,
 // the scales are fixed (fp16 plane below 2^14, e4m3 copy two binades below saturation) and the layer is run again so the
 // next one sees its final input.  Synchronises per layer; happens once (first forward, or after "recalibrate").
-static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, const int *sizes, int B, int H, int W, const NetLayout &L,
-                           char *ws, void *stream) {
+static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, const int *sizes, int B, const NetLayout &L, char *ws,
+                           void *stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  int h = H, w = W;
   for (int l = 0; l < 13; ++l) {
-    const void *in = l == 0 ? images : (const void *)(ws + L.act[l - 1]);
-    if (L.stack && l == 9)      // pad rows of conv4_3's stacked output (see ctpn_net_forward)
-      CTPN_CUDA(cudaMemsetAsync(ws + L.act[9], 0, (size_t)n->planes * B * (L.h[9] + 1) * L.w[9] * kConvs[9].cout * 2, st));
+    const ConvLayer &c = L.conv[l];
     float s_try = 1.f;
     for (int attempt = 0; ; ++attempt) {
-      n->act_s[l] = s_try; n->act_t[l] = 1.f;
-      int rc = l == 0 ? conv1_1_tc_ragged(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, 2, true, s_try, 1.f, sizes, stream)
-                      : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, sizes, stream);
+      int rc = run_conv(n, L, l, images, src_is_f32, sizes, B, ws, s_try, 1.f, stream);
       if (rc) return rc;
-      const long long cnt = (long long)B * (L.h[l] + ((L.stack && l >= 9 && l <= 12) ? 1 : 0)) * L.w[l] * kConvs[l].cout;
       CTPN_CUDA(cudaMemsetAsync(n->absmax_dev, 0, sizeof(unsigned), st));
-      absmax_f16_kernel<<<1184, 256, 0, st>>>((const __half *)(ws + L.act[l]), cnt, n->absmax_dev);
+      absmax_f16_kernel<<<1184, 256, 0, st>>>((const __half *)(ws + c.out), c.elems, n->absmax_dev);
       CTPN_LAUNCH_CHECK();
       unsigned bits = 0;
       CTPN_CUDA(cudaMemcpyAsync(&bits, n->absmax_dev, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -338,11 +362,8 @@ static int calibrate_f16f8(ctpn_net *n, const void *images, int src_is_f32, cons
       n->act_t[l] = exp2f(floorf(log2f(448.f / amax)) - 2.f);    // two binades of headroom; beyond that e4m3 saturates (cross term only)
       break;
     }
-    int rc = l == 0 ? conv1_1_tc_ragged(images, src_is_f32, n->lut, n->c11_w, n->c11_b, ws + L.act[0], B, h, w, 2, true, n->act_s[0],
-                                        n->act_t[0], sizes, stream)
-                    : run_layer_f16f8(n, l, in, ws + L.act[l], B, h, w, L.stack, sizes, stream);
+    int rc = run_conv(n, L, l, images, src_is_f32, sizes, B, ws, n->act_s[l], n->act_t[l], stream);
     if (rc) return rc;
-    h = L.h[l]; w = L.w[l];
   }
   n->calibrated = true;
   return CTPN_OK;
@@ -374,8 +395,10 @@ extern "C" int ctpn_net_set_option(ctpn_net_t *net, const char *key, int value) 
   if (!strcmp(key, "keep_activations")) net->keep = value != 0;
   else if (!strcmp(key, "recalibrate")) net->calibrated = false;
 #ifdef CTPN_DEBUG   // float32 SIMT reference kernels: test library only
-  else if (!strcmp(key, "conv_simt")) net->conv_simt = value != 0;
-  else if (!strcmp(key, "conv1_simt")) net->conv1_simt = value != 0;
+  else if (!strcmp(key, "conv_simt")) {
+    CTPN_REQUIRE(!value || !net->f16f8, "ctpn_net_set_option: the SIMT reference kernels read bf16 planes, not F16F8");
+    net->conv_simt = value != 0;
+  }
 #endif
   else { set_error("ctpn_net_set_option: unknown key '%s'", key); return CTPN_ERR_INVALID; }
   return CTPN_OK;
@@ -405,7 +428,7 @@ extern "C" size_t ctpn_net_workspace_bytes(const ctpn_net_t *net, int B, int H, 
 static int net_forward(ctpn_net *net, const void *images, int src_is_f32, const int *sizes, int B, int H, int W,
                        float *cls_score_out, float *bbox_pred_out, void *workspace, size_t workspace_bytes, void *stream) {
 #ifdef CTPN_DEBUG
-  CTPN_REQUIRE(!sizes || !(net->conv_simt || net->conv1_simt), "ctpn_net_forward_ragged: the SIMT reference kernels take uniform batches only");
+  CTPN_REQUIRE(!sizes || !net->conv_simt, "ctpn_net_forward_ragged: the SIMT reference kernels take uniform batches only");
 #endif
   int rc = finalize(net);
   if (rc) return rc;
@@ -417,71 +440,33 @@ static int net_forward(ctpn_net *net, const void *images, int src_is_f32, const 
   char *ws = (char *)workspace;
   const int P = net->planes;
   net->taps.clear();
-  if (net->f16f8) {
-    // 2-unit arithmetic: conv1_1 and the thirteen 3x3 layers on F16F8 planes (calibrated on the first batch)
-    if (!net->calibrated && (rc = calibrate_f16f8(net, images, src_is_f32, sizes, B, H, W, L, ws, stream))) return rc;
-    int hh = H, ww = W;
-    if ((rc = conv1_1_tc_ragged(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, 2, true, net->act_s[0],
-                                net->act_t[0], sizes, stream))) return rc;
-    net->taps["conv1_1"] = Tap{ws + L.act[0], (long long)B * H * W, 64, true, net->act_s[0], net->act_t[0]};
-    for (int l = 1; l < 14; ++l) {
-      if (L.stack && l == 9)      // conv4_3 writes only the image rows of its stacked output: the pad rows must be zero
-        CTPN_CUDA(cudaMemsetAsync(ws + L.act[9], 0, (size_t)P * B * (L.h[9] + 1) * L.w[9] * kConvs[9].cout * 2, (cudaStream_t)stream));
-      if ((rc = run_layer_f16f8(net, l, ws + L.act[l - 1], ws + L.act[l], B, hh, ww, L.stack, sizes, stream))) return rc;
-      hh = L.h[l]; ww = L.w[l];
-      const ConvSpec &s = kConvs[l];
-      const bool stacked = L.stack && l >= 9 && l <= 12;
-      net->taps[s.pool ? std::string(s.name) + "+pool" : std::string(s.name)] =
-          Tap{ws + L.act[l], (long long)B * hh * ww, s.cout, true, l == 13 ? 0.f : net->act_s[l], l == 13 ? 0.f : net->act_t[l],
-              stacked ? hh : 0, stacked ? ww : 0};
-    }
-  }
-  auto conv1 = [&](const void *src, int f32, const float *lut, const float *w, const float *b, void *out, int B_, int H_, int W_, int P_,
-                   void *st) {
-#ifdef CTPN_DEBUG
-    if (net->conv_simt || net->conv1_simt) return ctpn_conv1_1(src, f32, lut, w, b, out, B_, H_, W_, P_, st);
-#endif
-    return conv1_1_tc_ragged(src, f32, lut, w, b, out, B_, H_, W_, P_, false, 1.f, 1.f, sizes, st);
-  };
-  // 3x3 layers pass the extents (output level `lvl`); the 1x1 matmuls run on the whole canvas (sizes = null)
-  auto conv3 = [&](const void *in, const void *w, const float *b, void *out, int B_, int H_, int W_, int cin, int cout, int taps, int P_,
-                   int flags, const int *sz, int lvl, void *st) {
-#ifdef CTPN_DEBUG
-    if (net->conv_simt) return ctpn_conv3x3_simt(in, w, b, out, B_, H_, W_, cin, cout, taps, P_, flags, st);
-#endif
-    return conv3x3_ragged(in, w, b, out, B_, H_, W_, cin, cout, taps, P_, flags, sz, lvl, st);
-  };
-  const int pf = net->promote ? CTPN_F_PROMOTE : 0;     // CTPN_ARITH_BF16X3P: every conv_tc layer below
-  if (!net->f16f8) {
-  if ((rc = conv1(images, src_is_f32, net->lut, net->c11_w, net->c11_b, ws + L.act[0], B, H, W, P, stream))) return rc;
-  net->taps["conv1_1"] = Tap{ws + L.act[0], (long long)B * H * W, 64, true};
-  int h = H, w = W;
-  for (int l = 1; l < 14; ++l) {
+  // F16F8: conv1_1 and the thirteen 3x3 layers on F16F8 planes, calibrated on the first batch
+  if (net->f16f8 && !net->calibrated && (rc = calibrate_f16f8(net, images, src_is_f32, sizes, B, L, ws, stream))) return rc;
+  for (int l = 0; l < 14; ++l) {
     const ConvSpec &s = kConvs[l];
-    int flags = CTPN_F_RELU | (s.pool ? CTPN_F_POOL : 0) | pf;
-    const bool stacked = L.stack && l >= 9 && l <= 12;
-    if (stacked) flags |= CTPN_F_STACK_OUT;
-    if (L.stack && l >= 10) flags |= CTPN_F_STACK_IN;
-    if (L.stack && l == 9)      // conv4_3 writes only the image rows of its stacked output: the pad rows must be zero
-      CTPN_CUDA(cudaMemsetAsync(ws + L.act[9], 0, (size_t)P * B * (L.h[9] + 1) * L.w[9] * kConvs[9].cout * 2, (cudaStream_t)stream));
-    if ((rc = conv3(ws + L.act[l - 1], net->conv_w[l], net->conv_b[l], ws + L.act[l], B, h, w, s.cin, s.cout, 9, P, flags, sizes,
-                    out_level(l), stream))) return rc;
-    h = L.h[l]; w = L.w[l];
+    const ConvLayer &c = L.conv[l];
+    if ((rc = run_conv(net, L, l, images, src_is_f32, sizes, B, ws, net->act_s[l], net->act_t[l], stream))) return rc;
+    const bool q = net->f16f8 && !(c.flags & CTPN_F_OUT_BF16X2);     // F16F8 output planes
     net->taps[s.pool ? std::string(s.name) + "+pool" : std::string(s.name)] =
-        Tap{ws + L.act[l], (long long)B * h * w, s.cout, true, 0.f, 0.f, stacked ? h : 0, stacked ? w : 0};
-  }
+        Tap{ws + c.out, (long long)B * c.ho * c.wo, s.cout, true, q ? net->act_s[l] : 0.f, q ? net->act_t[l] : 0.f,
+            c.stacked ? c.ho : 0, c.stacked ? c.wo : 0};
   }
   const int M = B * L.fh * L.fw;
+  const int pf = net->promote ? CTPN_F_PROMOTE : 0;     // CTPN_ARITH_BF16X3P: every matmul below
+  // the 1x1 matmuls run on the whole canvas (no extents)
   auto gemm = [&](const void *in, const void *w, const float *b, void *out, int cin, int cout, int flags) {
-    return conv3(in, w, b, out, 1, 1, M, cin, cout, 1, P, flags, nullptr, 0, stream);
+#ifdef CTPN_DEBUG
+    if (net->conv_simt) return ctpn_conv3x3_simt(in, w, b, out, 1, 1, M, cin, cout, 1, P, flags, stream);
+#endif
+    return conv_tc_run(in, w, b, out, 1, 1, M, cin, cout, 1, P, flags, nullptr, nullptr, 0, stream);
   };
-  if ((rc = gemm(ws + L.act[13], net->xproj_w, net->xproj_b, ws + L.xproj, 512, 1024, CTPN_F_OUT_F32 | pf))) return rc;
+  if ((rc = gemm(ws + L.conv[13].out, net->xproj_w, net->xproj_b, ws + L.xproj, 512, 1024, CTPN_F_OUT_F32 | pf))) return rc;
   net->taps["xproj"] = Tap{ws + L.xproj, M, 1024, false};
-  if ((rc = bilstm_ragged((const float *)(ws + L.xproj), net->wh_fw, net->wh_bw, ws + L.act[14], B * L.fh, L.fw, P, sizes, L.fh, stream))) return rc;
-  net->taps["lstm_out"] = Tap{ws + L.act[14], M, 256, true};
-  if ((rc = gemm(ws + L.act[14], net->fc_w, net->fc_b, ws + L.act[15], 256, 512, pf))) return rc;
-  net->taps["lstm_o"] = Tap{ws + L.act[15], M, 512, true};
-  if ((rc = gemm(ws + L.act[15], net->head_w, net->head_b, ws + L.heads, 512, 64, CTPN_F_OUT_F32 | pf))) return rc;
+  if ((rc = bilstm_ragged((const float *)(ws + L.xproj), net->wh_fw, net->wh_bw, ws + L.lstm, B * L.fh, L.fw, P, sizes, L.fh, stream))) return rc;
+  net->taps["lstm_out"] = Tap{ws + L.lstm, M, 256, true};
+  if ((rc = gemm(ws + L.lstm, net->fc_w, net->fc_b, ws + L.fc, 256, 512, pf))) return rc;
+  net->taps["lstm_o"] = Tap{ws + L.fc, M, 512, true};
+  if ((rc = gemm(ws + L.fc, net->head_w, net->head_b, ws + L.heads, 512, 64, CTPN_F_OUT_F32 | pf))) return rc;
   const long long tot = (long long)M * 64;
   split_heads_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float *)(ws + L.heads), M, cls_score_out, bbox_pred_out);
   CTPN_LAUNCH_CHECK();
@@ -514,13 +499,12 @@ extern "C" int ctpn_net_debug_tap(ctpn_net_t *net, const char *name, float *out_
   *count = (size_t)n;
   if (!out_f32) return CTPN_OK;
   CTPN_REQUIRE(capacity >= (size_t)n, "ctpn_net_debug_tap: buffer too small (%zu < %lld)", capacity, n);
+  const long long stored = t.stack_h ? n / t.stack_h * (t.stack_h + 1) : n;      // elements per plane incl. pad rows
   if (t.planes && t.q_s > 0.f) {
-    const long long stored = t.stack_h ? n / t.stack_h * (t.stack_h + 1) : n;      // elements per plane incl. pad rows
     f16f8_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const __half *)t.ptr, (const uint8_t *)t.ptr + stored * 2, n,
                                                                                        t.channels, t.q_s, t.q_t, t.stack_h, t.stack_w, out_f32);
     CTPN_LAUNCH_CHECK();
   } else if (t.planes) {
-    const long long stored = t.stack_h ? n / t.stack_h * (t.stack_h + 1) : n;      // elements per plane incl. pad rows
     planes_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)t.ptr, n, stored, net->planes, t.channels,
                                                                                         t.stack_h, t.stack_w, out_f32);
     CTPN_LAUNCH_CHECK();

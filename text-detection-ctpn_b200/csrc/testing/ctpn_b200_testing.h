@@ -2,8 +2,9 @@
  * Test-only entry points of libctpn_b200_dbg.so (tests/_native/): float32 SIMT reference kernels with the product
  * kernels' contracts, and a hardware probe.  None of this is in the product library libctpn_b200.so or in
  * include/ctpn_b200.h.  The debug library is the product sources compiled with -DCTPN_DEBUG (ablation switches
- * CTPN_TC_DEBUG / CTPN_C1_DEBUG, tuning overrides CTPN_TC_BN / CTPN_TC_STAGES_* / CTPN_TC_MCAST / CTPN_TC_PROMOTE, the "conv_simt" /
- * "conv1_simt" options of ctpn_net_set_option) plus the two files in this directory.
+ * CTPN_TC_DEBUG / CTPN_C1_DEBUG, tuning overrides CTPN_TC_BN / CTPN_TC_STAGES_* / CTPN_TC_MCAST / CTPN_TC_PROMOTE, the "conv_simt"
+ * option of ctpn_net_set_option, which runs every convolution and matmul of a bf16-plane net on the SIMT kernels below and is
+ * refused on an F16F8 net) plus the two files in this directory.
  */
 #ifndef CTPN_B200_TESTING_H_
 #define CTPN_B200_TESTING_H_
