@@ -26,7 +26,7 @@ __constant__ int c_anchor_y[2][10][2] = {
 };
 
 __device__ __forceinline__ uint32_t desc_key(float s) {
-  uint32_t u = __float_as_uint(s);
+  uint32_t u = __float_as_uint(s == 0.f ? 0.f : s);   // -0 ties with +0 (then ascending index), as in the oracle's sort
   uint32_t asc = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
   return ~asc;   // ascending key order == descending score
 }
