@@ -21,6 +21,7 @@
  *                        (the demo_pb.py:73-75 boundary), fed by lib/fast_rcnn/test.py:7-31
  *   ctpn_resize_linear_u8   cv2.resize in resize_im, ctpn/demo.py:21-25 (and draw_boxes :50)
  *   ctpn_image_blob_f32     _get_image_blob, lib/fast_rcnn/test.py:7-31 (float32 cv2.resize of the mean-subtracted image)
+ *   ctpn_resize_linear_u8_ragged / ctpn_image_blob_f32_ragged   the same two, for a batch of images of different sizes
  *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
@@ -218,6 +219,24 @@ int ctpn_resize_linear_u8(const void *src, int B, int sh, int sw, int channels, 
  * lut[256][3] = float32(double(v) - PIXEL_MEANS[c]) (device).  dst size from ctpn_resize_out_size. */
 int ctpn_image_blob_f32(const void *src_u8, const float *lut, int B, int sh, int sw, double fx, double fy, float *dst, int dh,
                         int dw, void *stream);
+
+/* Ragged forms of the two calls above: B images of different sizes and scales in one launch.  Image b is read from
+ * src + src_offset[b] (elements) as [h][pitch][C] with (h, w, pitch) = src_hwp[3b..3b+2] (pitch >= w pixels per row),
+ * resized by (fx, fy) = fxy[2b..2b+1] to dst_hw[2b..2b+1] (must equal ctpn_resize_out_size), and written to rows < dh,
+ * columns < dw of slice b of the canvas dst [B][H][W][C]; the rest of the canvas is NOT written.  Every image is
+ * bit-identical to the single-image call on that image alone (same per-pixel code, incl. the INTER_AREA routing of an
+ * exact 1/2 scale).  ctpn_image_blob_f32_ragged: C = 3, float32 canvas, lut as for ctpn_image_blob_f32.
+ * EXCEPTION to the pointer convention of this header: src_offset, src_hwp, fxy and dst_hw are small HOST arrays
+ * (1 <= B <= 64); src, dst and lut are device pointers, src_elems the number of elements src holds.  Every descriptor is
+ * validated before any CUDA call (CTPN_ERR_INVALID naming the image: dst_hw != cvRound size, output larger than the
+ * canvas, offset + ((h - 1) * pitch + w) * C > src_elems, pitch < w, a scale <= 0, a NULL pointer) and then passed to
+ * the kernel by value, so the kernel touches no memory whose extent the host did not check. */
+int ctpn_resize_linear_u8_ragged(const void *src, size_t src_elems, const long long *src_offset, const int *src_hwp,
+                                 const double *fxy, const int *dst_hw, int B, int channels, void *dst, int H, int W,
+                                 void *stream);
+int ctpn_image_blob_f32_ragged(const void *src_u8, size_t src_elems, const long long *src_offset, const int *src_hwp,
+                               const double *fxy, const int *dst_hw, const float *lut, int B, float *dst, int H, int W,
+                               void *stream);
 
 /* CRC-32C (Castagnoli) of a host buffer, continuing from `crc` (0 to start): the per-tensor checksum of TF checkpoint V2
  * files, used by the weight importer (ctpn_b200/tf_import.py) to verify every tensor it loads. */

@@ -6,7 +6,8 @@ ctpn(sess, net, image_name) keeps the reference signature (demo.py:55-68): read 
 (short side 600, long side <= 1200), test_ctpn, TextDetector, write data/results/res_<stem>.txt
 and the annotated image.  `sess` is a ctpn_b200.Session (replaces tf.Session + Saver.restore).
 --batch N > 1 runs N images at a time through Engine.rois_ragged (images of different sizes in one batch), with the same
-resize, blob, TextDetector and output files per image (ctpn_batch).
+resize, blob, TextDetector and output files per image (ctpn_batch).  --device-frontend (with --batch N) runs the resize
+and the blob on the GPU as well (Engine.rois_images, ctpn_batch_device); the output files are the same.
 """
 from __future__ import print_function
 
@@ -99,6 +100,23 @@ def ctpn_batch(sess, image_names):
     print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
 
 
+def ctpn_batch_device(sess, image_names):
+    """ctpn_batch with resize_im and _get_image_blob on the device (Engine.rois_images): the images go up as read, and
+    the resized images come back for draw_boxes.  Same TextDetector, draw_boxes and output files per image."""
+    timer = Timer()
+    timer.tic()
+    imgs = [cv2.imread(name) for name in image_names]
+    res = sess.engine.rois_images(imgs, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
+    for name, (r, im_scale, scale, img) in zip(image_names, res):
+        scores, boxes = r[:, 0], r[:, 1:5] / np.float64(im_scale)      # the float64 division of test_ctpn
+        textdetector = TextDetector(native=NATIVE_CONNECTOR)
+        boxes = textdetector.detect(boxes, scores[:, np.newaxis], img.shape[:2])
+        draw_boxes(img, name, boxes, scale)
+        print('{:s}: {:d} text lines'.format(name, boxes.shape[0]))
+    timer.toc()
+    print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--weights", default=None,
@@ -111,7 +129,12 @@ def main(argv=None):
                     help="build the text lines with the library's C++ connector (same lines, float32-rounding agreement)")
     ap.add_argument("--batch", type=int, default=1,
                     help="images per ragged batch (Engine.detect_ragged); 1 = one image at a time through test_ctpn")
+    ap.add_argument("--device-frontend", action="store_true",
+                    help="with --batch N: run resize_im and the image blob on the GPU (Engine.rois_images) instead of cv2 on "
+                         "the host; same output files")
     args = ap.parse_args(argv)
+    if args.device_frontend and args.batch <= 1:
+        ap.error("--device-frontend needs --batch N with N > 1")
     global NATIVE_CONNECTOR
     NATIVE_CONNECTOR = args.native_connector
     if os.path.exists(RESULTS_DIR):
@@ -138,7 +161,7 @@ def main(argv=None):
     if args.batch > 1:
         for k in range(0, len(names), args.batch):
             print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')
-            ctpn_batch(sess, names[k:k + args.batch])
+            (ctpn_batch_device if args.device_frontend else ctpn_batch)(sess, names[k:k + args.batch])
         return
     for im_name in names:
         print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')

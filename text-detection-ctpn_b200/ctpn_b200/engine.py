@@ -7,6 +7,7 @@ compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
     scores, boxes = eng.detect(im)               # == lib.fast_rcnn.test.test_ctpn
     results = eng.detect_batch(uint8_batch)      # [B,H,W,3] -> list of (scores, boxes)
     results = eng.detect_ragged([im0, im1, ...])  # images of different sizes, batched on shared canvases
+    results = eng.detect_images([photo0, ...])   # raw photos: resize_im + _get_image_blob on the device, then as above
 
 `planes` / `mode` select the arithmetic of the tensor-core layers (see include/ctpn_b200.h); accumulation is always
 float32:  1 / "bf16" = bf16 operands (1 unit per MAC);  2 / "bf16x2" = bf16x2 split, ~16 mantissa bits (3 units);
@@ -16,6 +17,7 @@ main accumulator promoted to round-to-nearest float32 every 64 channels of a tap
 4 / "f16f8" = fp16 operands + e4m3 cross terms for the 3x3 layers (2 units; head logits within 1e-3 of float32, 6-8e-4
 measured; activation scales calibrated on the first batch).
 """
+import collections
 import ctypes as C
 
 import os
@@ -568,6 +570,13 @@ class Engine:
                                             N.stream_ptr()), "ctpn_resize_linear_u8")
         return out
 
+    def _mean_lut(self):
+        """Device float32 [256,3]: float32(double(v) - PIXEL_MEANS[c]), the mean subtraction of _get_image_blob."""
+        if getattr(self, "_lut", None) is None:
+            means = np.array([102.9801, 115.9465, 122.7717])              # cfg.PIXEL_MEANS (config.py:200), BGR
+            self._lut = torch.from_numpy((np.arange(256, dtype=np.float64)[:, None] - means[None, :]).astype(np.float32)).to(self.device)
+        return self._lut
+
     def image_blob(self, images, im_scale):
         """_get_image_blob (lib/fast_rcnn/test.py:7-31) on the device for a same-shape uint8 BGR batch [B,H,W,3]: mean
         subtraction (float32(double(v) - PIXEL_MEANS)) fused with the float32 cv2.resize by im_scale.  Returns a float32
@@ -578,9 +587,7 @@ class Engine:
             raise ValueError("image_blob expects a uint8 [B,H,W,3] batch")
         t = t.to(self.device, non_blocking=True).contiguous()
         B, H, W, _ = t.shape
-        if getattr(self, "_lut", None) is None:
-            means = np.array([102.9801, 115.9465, 122.7717])              # cfg.PIXEL_MEANS (config.py:200), BGR
-            self._lut = torch.from_numpy((np.arange(256, dtype=np.float64)[:, None] - means[None, :]).astype(np.float32)).to(self.device)
+        self._mean_lut()
         dh, dw = C.c_int(0), C.c_int(0)
         N.check(N.lib.ctpn_resize_out_size(H, W, float(im_scale), float(im_scale), C.byref(dh), C.byref(dw)), "ctpn_resize_out_size")
         out = torch.empty((B, dh.value, dw.value, 3), dtype=torch.float32, device=self.device)
@@ -616,6 +623,78 @@ class Engine:
         resized = images if f == 1.0 else self.resize_images(images, f)
         return self.detect_batch(resized), f
 
+    def rois_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200):
+        """The front half of ctpn() (demo.py:59-61) plus test_ctpn for a list of raw HxWx3 uint8 BGR images of any sizes,
+        front-end on the device: resize_im (short side -> scale, long side <= max_scale; resize=False: the images are
+        already at that scale) and _get_image_blob (uint8 when im_scale == 1, else the mean-subtracted float32 rescale),
+        then ragged batches of at most max_batch (frontend_plan + ragged_plan).  Each batch's sources travel in one pinned
+        H2D copy; ctpn_resize_linear_u8_ragged writes the uint8 canvas (or, for float32 batches, a uint8 canvas that
+        ctpn_image_blob_f32_ragged turns into the float32 blob canvas), and detect_packed runs the batch with per-image
+        extents.  Returns, in input order, (rois float32 [n,5] in blob coordinates, im_scale, f) per image -- and the
+        resize_im output as a host uint8 array as a 4th item with return_resized (what draw_boxes draws on).  Every image
+        is bit-identical to the host front-end with OpenCV's own code (IPP-dispatching cv2 builds differ on float
+        rescales) followed by detect on that image alone.  Raises ValueError on a bad image (see frontend_plan)."""
+        if not 1 <= int(max_batch) <= 64:
+            raise ValueError("rois_images: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)")
+        images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
+        plan = frontend_plan(images, resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg)
+        out = [None] * len(images)
+        rows = self.result_rows()
+        lut = self._mean_lut()
+        stream = N.stream_ptr()
+        for idxs, (H, W) in ragged_plan([p.blob for p in plan], [p.dtype for p in plan], max_batch):
+            B = len(idxs)
+            items = [plan[i] for i in idxs]
+            nbytes = [images[i].size for i in idxs]
+            offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
+            total = int(sum(nbytes))
+            pinned = self._pin("frontend_src", (1 << max(20, (total - 1).bit_length()),), torch.uint8)   # grow-only sizes
+            pn = pinned.numpy()
+            for k, i in enumerate(idxs):
+                h, w = images[i].shape[:2]
+                pn[offsets[k]:offsets[k] + nbytes[k]].reshape(h, w, 3)[...] = images[i]
+            src = self._workspace("frontend_src", total)
+            src[:total].copy_(pinned[:total], non_blocking=True)           # the batch's one H2D
+            hwp = np.array([images[i].shape[:2] + (images[i].shape[1],) for i in idxs], np.int32)
+            fxy = np.array([[p.f, p.f] for p in items], np.float64)
+            is_u8 = items[0].dtype == "|u1"
+            if is_u8:          # im_scale == 1: resize_im writes the network's uint8 canvas directly
+                u8 = canvas = torch.empty((B, H, W, 3), dtype=torch.uint8, device=self.device)
+                Hr, Wr = H, W
+            else:
+                Hr, Wr = max(p.resized[0] for p in items), max(p.resized[1] for p in items)
+                u8 = self._workspace("frontend_u8", B * Hr * Wr * 3)[:B * Hr * Wr * 3].view(B, Hr, Wr, 3)
+                canvas = torch.empty((B, H, W, 3), dtype=torch.float32, device=self.device)
+            resized_hw = np.array([p.resized for p in items], np.int32)
+            N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(src), total, N.ptr(offsets), N.ptr(hwp), N.ptr(fxy), N.ptr(resized_hw),
+                                                       B, 3, N.ptr(u8), Hr, Wr, stream), "ctpn_resize_linear_u8_ragged")
+            if not is_u8:
+                boffs = np.arange(B, dtype=np.int64) * (Hr * Wr * 3)
+                bhwp = np.concatenate([resized_hw, np.full((B, 1), Wr, np.int32)], axis=1)
+                bfxy = np.array([[p.im_scale, p.im_scale] for p in items], np.float64)
+                blob_hw = np.array([p.blob for p in items], np.int32)
+                N.check(N.lib.ctpn_image_blob_f32_ragged(N.ptr(u8), B * Hr * Wr * 3, N.ptr(boffs), N.ptr(bhwp), N.ptr(bfxy),
+                                                         N.ptr(blob_hw), N.ptr(lut), B, N.ptr(canvas), H, W, stream),
+                        "ctpn_image_blob_f32_ragged")
+            info_h = self._pin("info", (B, 3), torch.float32)
+            info_h.numpy()[...] = [[p.blob[0], p.blob[1], p.im_scale] for p in items]
+            packed = self.detect_packed(canvas, info_h.to(self.device, non_blocking=True), sizes=np.array([p.blob for p in items]))
+            out_h = self._pin("out", tuple(packed.shape), torch.float32)
+            out_h.copy_(packed, non_blocking=True)
+            resized = [u8[k, :p.resized[0], :p.resized[1]].cpu().numpy() for k, p in enumerate(items)] if return_resized else None
+            torch.cuda.current_stream().synchronize()              # also frees the pinned sources for the next batch
+            for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, B, rows))):
+                out[i] = (r, plan[i].im_scale, plan[i].f) + ((resized[k],) if return_resized else ())
+        return out
+
+    def detect_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200):
+        """rois_images as test_ctpn returns it: per image (scores float32 [n], boxes float64 [n,4] = rois / im_scale, f), plus
+        the resize_im output with return_resized.  Boxes are in the resize_im frame, as TextDetector expects them
+        (draw_boxes divides by f)."""
+        res = self.rois_images(images, resize=resize, max_batch=max_batch, return_resized=return_resized, scale=scale,
+                               max_scale=max_scale)
+        return [(r[0][:, 0], r[0][:, 1:5] / np.float64(r[1])) + tuple(r[2:]) for r in res]
+
     def detect(self, image, im_scale=1.0):
         """Single image [H,W,3] -> (scores, boxes); the test_ctpn() contract."""
         return self.detect_batch(image[None], im_scale)[0]
@@ -641,6 +720,58 @@ def ragged_plan(shapes, dtypes, max_batch=32):
             part = idxs[k:k + max_batch]
             plan.append((part, (max(int(shapes[i][0]) for i in part), max(int(shapes[i][1]) for i in part))))
     return plan
+
+
+FrontendStep = collections.namedtuple("FrontendStep", "f resized im_scale blob dtype")
+
+
+def _cv_round_size(h, w, s):
+    return int(np.rint(float(h) * s)), int(np.rint(float(w) * s))        # cvRound: round half to even, in float64
+
+
+def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None):
+    """What the demo's host front-end does to each image, computed on the host: shapes is a list of HxWx3 uint8 images
+    (anything with .shape and .dtype) or of (H, W[, 3]) tuples.  Per image a FrontendStep of
+      f         the resize_im factor (ctpn/demo.py: short side -> scale unless the long side would exceed max_scale;
+                1.0 with resize=False, for images already at that scale),
+      resized   its (h, w) as cv2.resize computes it (cvRound),
+      im_scale  _get_image_blob's scale (lib/fast_rcnn/test.py _im_scale: SCALES[0] / short side, or MAX_SIZE / long side
+                when np.round(im_scale * long side) > MAX_SIZE; cfg: SCALES and MAX_SIZE, default DEFAULT_CFG),
+      blob      the (h, w) of the blob the network sees,
+      dtype     '|u1' when im_scale == 1 (the uint8 image is the blob), else '<f4' (the float32 rescale).
+    Raises ValueError when an image is not HxWx3 uint8, a resize would be empty or a blob side would be under 16."""
+    c = dict(DEFAULT_CFG)
+    if cfg:
+        c.update(cfg)
+    target, max_size = float(c["SCALES"][0]), float(c["MAX_SIZE"])
+    out = []
+    for i, s in enumerate(shapes):
+        if hasattr(s, "shape") and hasattr(s, "dtype"):
+            if len(s.shape) != 3 or s.shape[2] != 3 or str(s.dtype) not in ("uint8", "torch.uint8"):
+                raise ValueError("frontend_plan: image %d must be HxWx3 uint8 (got %s %s)" % (i, tuple(s.shape), s.dtype))
+            s = tuple(s.shape)
+        s = tuple(int(v) for v in s)
+        if len(s) not in (2, 3) or (len(s) == 3 and s[2] != 3):
+            raise ValueError("frontend_plan: image %d must be HxWx3 uint8 (got shape %s)" % (i, s))
+        h, w = s[:2]
+        if h < 1 or w < 1:
+            raise ValueError("frontend_plan: image %d is empty (%dx%d)" % (i, h, w))
+        f = 1.0
+        if resize:
+            f = float(scale) / min(h, w)
+            if max_scale is not None and f * max(h, w) > max_scale:
+                f = float(max_scale) / max(h, w)
+        rh, rw = _cv_round_size(h, w, f)
+        if rh < 1 or rw < 1:
+            raise ValueError("frontend_plan: image %d (%dx%d) resizes to nothing at f = %r" % (i, h, w, f))
+        im_scale = target / float(min(rh, rw))
+        if np.round(im_scale * max(rh, rw)) > max_size:
+            im_scale = max_size / float(max(rh, rw))
+        bh, bw = (rh, rw) if im_scale == 1.0 else _cv_round_size(rh, rw, im_scale)
+        if bh < 16 or bw < 16:
+            raise ValueError("frontend_plan: image %d (%dx%d) gives a %dx%d blob; both sides must be at least 16" % (i, h, w, bh, bw))
+        out.append(FrontendStep(f, (rh, rw), im_scale, (bh, bw), "|u1" if im_scale == 1.0 else "<f4"))
+    return out
 
 
 # the 38 variables of the VGGnet_test graph (SURVEY.md App. A.2); a TF checkpoint also holds optimizer slots etc.
