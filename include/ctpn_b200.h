@@ -22,7 +22,7 @@
  *   ctpn_resize_linear_u8   cv2.resize in resize_im, ctpn/demo.py:21-25 (and draw_boxes :50)
  *   ctpn_image_blob_f32     _get_image_blob, lib/fast_rcnn/test.py:7-31 (float32 cv2.resize of the mean-subtracted image)
  *   ctpn_resize_linear_u8_ragged / ctpn_image_blob_f32_ragged   the same two, for a batch of images of different sizes
- *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host
+ *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host / ctpn_text_lines (batched, device)
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
  *                        text_proposal_connector.py:21-64 and text_proposal_connector_oriented.py:24-105
@@ -242,8 +242,28 @@ int ctpn_image_blob_f32_ragged(const void *src_u8, size_t src_elems, const long 
  * files, used by the weight importer (ctpn_b200/tf_import.py) to verify every tensor it loads. */
 uint32_t ctpn_crc32c_host(const void *data, size_t n, uint32_t crc);
 
-/* ---- text lines on the host (replaces lib/text_connector/detectors.py:19-49 and the connector classes) ----
- * TextDetector.detect in C++ on the CPU: score filter (> 0.7), score order, NMS 0.2, proposal graph
+/* ---- text lines (replaces lib/text_connector/detectors.py:19-49 and the connector classes) ----
+ * Two connectors with one arithmetic (csrc/textline.cuh: the same __host__ __device__ functions, no FMA contraction, IEEE
+ * division and sqrt): ctpn_text_lines_host on the CPU for one image, ctpn_text_lines on the device for a batch.  Their
+ * lines are equal as float64 bits.
+ *
+ * ctpn_text_lines: the connector for a batch of the proposal layer's outputs, where they lie on the device.
+ *   rois [batch][rows][5] (score, x1, y1, x2, y2) in blob coordinates and counts [batch] (valid rows per image) are device
+ *   arrays in ctpn_proposals' layout; the rows may come in any order.  im_hw [batch][2] (h, w: the frame of the lines, i.e.
+ *   the resize_im output) and im_scale [batch] (the blob scale) are small HOST arrays (1 <= batch <= 64), validated
+ *   before any CUDA call.  For every image b, num_lines[b] and the first num_lines[b] rows of lines_out[b] ([batch][rows][9]
+ *   float64, device) equal ctpn_text_lines_host on boxes = float32(double(roi[1:5]) / im_scale[b]) (test_ctpn's
+ *   rois / np.float64(im_scale) stored as float32), scores = roi[0], size im_hw[b], with the same oriented and cfg9.
+ *   Rows of lines_out[b] past num_lines[b] are not written.  Every line starts at a distinct chain head, which is one of
+ *   the counts[b] <= rows proposals, so rows lines per image always suffice.
+ *   status [batch] (device): 0, 1 where ctpn_text_lines_host would fail because a surviving proposal's x1 lies outside
+ *   [0, w) (the reference raises IndexError; the kernel never reads outside its column table), 2 where counts[b] is not
+ *   in [0, rows]; num_lines[b] is 0 for a nonzero status and the other images are unaffected.
+ *   0 <= rows <= 65536; every per-image array lives in the workspace (ctpn_text_lines_workspace_bytes(batch, rows, max w),
+ *   O(rows^2 / 8) bytes per image for the NMS bitmask), CTPN_ERR_INVALID when it is smaller or an argument is bad.
+ *   Stream-ordered, no allocation, no synchronisation; CTPN_ERR_NO_DEVICE without a GPU.
+ *
+ * ctpn_text_lines_host: TextDetector.detect in C++ on the CPU: score filter (> 0.7), score order, NMS 0.2, proposal graph
  * (text_proposal_graph_builder.py:6-78), chains (other.py:16-29), horizontal (oriented = 0,
  * text_proposal_connector.py:13-64) or oriented (1, text_proposal_connector_oriented.py:24-105) line fitting and
  * filter_boxes.  proposals [n][4] and scores [n] are test_ctpn()'s output (host memory); lines_out receives
@@ -252,6 +272,10 @@ uint32_t ctpn_crc32c_host(const void *data, size_t n, uint32_t crc);
  * min_num_proposals).  CTPN_ERR_INVALID (with *num_lines set) when more than max_lines lines were found. */
 int ctpn_text_lines_host(const float *proposals, const float *scores, int n, int im_h, int im_w, int oriented,
                          const float *cfg9, double *lines_out, int max_lines, int *num_lines);
+size_t ctpn_text_lines_workspace_bytes(int batch, int rows, int max_im_w);
+int ctpn_text_lines(const float *rois, const int *counts, int batch, int rows, const int *im_hw, const double *im_scale,
+                    int oriented, const float *cfg9, double *lines_out, int *num_lines, int *status, void *workspace,
+                    size_t workspace_bytes, void *stream);
 
 /* The stages of ctpn_text_lines_host for callers that fit the lines themselves (the Python TextDetector mirror fits with
  * numpy so that np.polyfit's own LAPACK solve produces the coordinates).

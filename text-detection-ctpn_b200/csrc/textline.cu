@@ -7,137 +7,27 @@
 //   oriented lines            lib/text_connector/text_proposal_connector_oriented.py:24-105
 //
 // Pure CPU code (no device work): the Python connector (with its NMS) costs 4-9 ms per image, this one 0.1-0.4 ms, so
-// it keeps up with the GPU part of the pipeline from one host thread.  Arithmetic follows what numpy >= 2 does in
+// it keeps up with the GPU part of the pipeline from one host thread.  The per-element arithmetic lives in textline.cuh,
+// shared with the batched device connector (textline_device.cu).  Arithmetic follows what numpy >= 2 does in
 // the reference's expressions: float32 wherever both operands are float32 (python-float constants are "weak"),
 // numpy's pairwise summation for contiguous float32 reductions, np.polyfit / np.poly1d in float64 (np.vander promotes
 // the float32 abscissae), one rounding to float32 when a fitted value is stored into the float32 line table.
 // Agreement with the Python mirror / the reference: identical line sets; coordinates within float32 rounding
 // (tests/test_textline_cpu.py states the tolerance and reports the bit-exact fraction).
 #include <algorithm>
-#include <cmath>
 #include <cstdint>
 #include <cstring>
-#include <numeric>
 #include <vector>
 
 #include "common.cuh"
+#include "textline.cuh"
 
 namespace ctpn {
 namespace {
 
-struct TextCfg {
-  float min_score = 0.7f, nms_thresh = 0.2f, min_v_overlaps = 0.7f, min_size_sim = 0.7f;
-  int max_gap = 50;
-  double min_ratio = 0.5, line_min_score = 0.9;
-  int proposal_width = 16, min_num_proposals = 2;
-};
-
-struct Box { float x1, y1, x2, y2; };
-
-// numpy's float32 add.reduce over a contiguous vector (pairwise summation, 8 accumulators per <= 128-element block)
-float pairwise_sum_f32(const float *a, size_t n) {
-  if (n < 8) {
-    float res = 0.f;
-    for (size_t i = 0; i < n; ++i) res += a[i];
-    return res;
-  }
-  if (n <= 128) {
-    float r[8];
-    for (int j = 0; j < 8; ++j) r[j] = a[j];
-    size_t i;
-    for (i = 8; i < n - (n % 8); i += 8)
-      for (int j = 0; j < 8; ++j) r[j] += a[i + j];
-    float res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
-    for (; i < n; ++i) res += a[i];
-    return res;
-  }
-  size_t n2 = n / 2;
-  n2 -= n2 % 8;
-  return pairwise_sum_f32(a, n2) + pairwise_sum_f32(a + n2, n - n2);
-}
-float np_sum_f32(const std::vector<float> &v) {
-  return pairwise_sum_f32(v.data(), v.size());
-}
-
-float iou_plus1(const Box &a, float area_a, const Box &b, float area_b) {
-  const float xx1 = std::max(a.x1, b.x1), yy1 = std::max(a.y1, b.y1);
-  const float xx2 = std::min(a.x2, b.x2), yy2 = std::min(a.y2, b.y2);
-  const float w = std::max(0.0f, xx2 - xx1 + 1.0f), h = std::max(0.0f, yy2 - yy1 + 1.0f);
-  const float inter = w * h;
-  return inter / (area_a + area_b - inter);
-}
-
-// np.polyfit(X, Y, 1) on float32 data.  numpy.vander promotes the float32 abscissae with `int`, i.e. to float64, so the
-// whole fit runs in double: column scaling by sqrt((lhs * lhs).sum(axis=0)), least squares (LAPACK gelsd in numpy; a
-// 2-column QR here -- both are accurate to ~1e-16, far below the float32 rounding applied when the result is stored),
-// coefficients divided by the scales.
-void polyfit1(const std::vector<float> &X, const std::vector<float> &Y, double &slope, double &icpt) {
-  const size_t n = X.size();
-  double s0 = 0.0, s1 = 0.0;                      // row-by-row accumulation of the axis-0 sum
-  for (size_t i = 0; i < n; ++i) {
-    s0 += (double)X[i] * (double)X[i];
-    s1 += 1.0;
-  }
-  const double scale0 = std::sqrt(s0), scale1 = std::sqrt(s1);
-  std::vector<double> u(n), w(n);
-  const double v = 1.0 / scale1;
-  for (size_t i = 0; i < n; ++i) u[i] = (double)X[i] / scale0;
-  // modified Gram-Schmidt QR of [u v]: well conditioned after the column scaling
-  double nu = 0;
-  for (size_t i = 0; i < n; ++i) nu += u[i] * u[i];
-  nu = std::sqrt(nu);
-  double r01 = 0;
-  for (size_t i = 0; i < n; ++i) r01 += (u[i] / nu) * v;
-  double nv = 0, qty0 = 0, qty1 = 0;
-  for (size_t i = 0; i < n; ++i) {
-    w[i] = v - r01 * (u[i] / nu);
-    nv += w[i] * w[i];
-  }
-  nv = std::sqrt(nv);
-  for (size_t i = 0; i < n; ++i) {
-    qty0 += (u[i] / nu) * (double)Y[i];
-    qty1 += (w[i] / nv) * (double)Y[i];
-  }
-  const double c1 = qty1 / nv;
-  const double c0 = (qty0 - r01 * c1) / nu;
-  slope = c0 / scale0;
-  icpt = c1 / scale1;
-}
-
-// fit_y (text_proposal_connector.py:13-19): Y at x1 and x2 on the fitted line.  np.poly1d evaluates float64
-// coefficients at the float32 abscissa in double; the caller rounds to float32 when it stores into text_lines.
-void fit_y(const std::vector<float> &X, const std::vector<float> &Y, float x1, float x2, double &y1, double &y2) {
-  bool all_same = true;
-  for (float x : X) all_same = all_same && (x == X[0]);
-  if (all_same) {
-    y1 = y2 = (double)Y[0];
-    return;
-  }
-  if (X.size() == 2) {
-    // two boxes: the least-squares line passes through both points.  Evaluated as an interpolation in double, every
-    // step is exact for float32 inputs in the connector's geometry (abscissa ratio 8/16, 24/16, ...), so the stored
-    // float32 value is the correctly rounded exact fit; numpy's LAPACK result carries ~1e-16 of noise, which decides
-    // the rounding when the exact value is a float32 tie (the mean of two adjacent-parity ordinates).
-    const double xa = X[0], xb = X[1], ya = Y[0], yb = Y[1];
-    y1 = ya + (yb - ya) * (((double)x1 - xa) / (xb - xa));
-    y2 = ya + (yb - ya) * (((double)x2 - xa) / (xb - xa));
-    return;
-  }
-  double m, c;
-  polyfit1(X, Y, m, c);
-  y1 = m * (double)x1 + c;
-  y2 = m * (double)x2 + c;
-}
-
-TextCfg parse_cfg(const float *cfg9) {
-  TextCfg cfg;
-  if (cfg9) {   // (min_score, nms_thresh, max_gap, min_v_overlaps, min_size_sim, min_ratio, line_min_score, width, min_num)
-    cfg.min_score = cfg9[0]; cfg.nms_thresh = cfg9[1]; cfg.max_gap = (int)cfg9[2]; cfg.min_v_overlaps = cfg9[3];
-    cfg.min_size_sim = cfg9[4]; cfg.min_ratio = (double)cfg9[5]; cfg.line_min_score = (double)cfg9[6];
-    cfg.proposal_width = (int)cfg9[7]; cfg.min_num_proposals = (int)cfg9[8];
-  }
-  return cfg;
-}
+using tl::Box;
+using tl::TextCfg;
+using tl::parse_cfg;
 
 // detectors.py:21-28: score filter, score-descending order (index ascending on ties), greedy NMS (IoU with the +1
 // convention, strict >).  Returns the surviving input indices in visiting order.
@@ -151,17 +41,15 @@ std::vector<int> filter_sort_nms(const float *proposals, const float *scores, in
   for (size_t k = 0; k < order.size(); ++k) {
     const float *p = proposals + 4 * (size_t)order[k];
     sb[k] = {p[0], p[1], p[2], p[3]};
-    area[k] = (p[2] - p[0] + 1.0f) * (p[3] - p[1] + 1.0f);
+    area[k] = tl::area_plus1(sb[k]);
   }
   std::vector<int> keep;
   std::vector<char> dead(sb.size(), 0);
   for (size_t i = 0; i < sb.size(); ++i) {
     if (dead[i]) continue;
     keep.push_back(order[i]);
-    for (size_t j = i + 1; j < sb.size(); ++j) {
-      if (dead[j] || sb[j].x1 > sb[i].x2 + 1.0f || sb[j].x2 + 1.0f < sb[i].x1) continue;   // no overlap: IoU = 0
-      if (iou_plus1(sb[i], area[i], sb[j], area[j]) > cfg.nms_thresh) dead[j] = 1;
-    }
+    for (size_t j = i + 1; j < sb.size(); ++j)
+      if (!dead[j] && tl::nms_suppresses(sb[i], area[i], sb[j], area[j], cfg.nms_thresh)) dead[j] = 1;
   }
   return keep;
 }
@@ -172,62 +60,25 @@ int build_chains(const std::vector<Box> &tp, const std::vector<float> &sc, int i
                  std::vector<int> &next, std::vector<char> &has_in) {
   const int m = (int)tp.size();
   for (int i = 0; i < m; ++i)
-    CTPN_REQUIRE(tp[i].x1 >= 0.f && (int)tp[i].x1 < im_w, "text lines: proposal x1=%g outside the image width %d",
+    CTPN_REQUIRE(tl::column_ok(tp[i].x1, im_w), "text lines: proposal x1=%g outside the image width %d",
                  (double)tp[i].x1, im_w);   // the reference would raise IndexError on boxes_table[int(x1)]
-  std::vector<float> heights(m);
-  std::vector<std::vector<int>> table(im_w);
-  for (int i = 0; i < m; ++i) {
-    heights[i] = tp[i].y2 - tp[i].y1 + 1.0f;
-    table[(int)tp[i].x1].push_back(i);
-  }
-  auto compatible = [&](int a, int b) {   // meet_v_iou(a, b): graph_builder.py:40-54
-    const float h1 = heights[a], h2 = heights[b];
-    const float y0 = std::max(tp[b].y1, tp[a].y1), y1 = std::min(tp[b].y2, tp[a].y2);
-    const float ov = std::max(0.0f, y1 - y0 + 1.0f) / std::min(h1, h2);
-    const float sim = std::min(h1, h2) / std::max(h1, h2);
-    return ov >= cfg.min_v_overlaps && sim >= cfg.min_size_sim;
-  };
-  std::vector<int> hits;
-  auto successions = [&](int i) {
-    const int x = (int)tp[i].x1;
-    for (int left = x + 1; left < std::min(x + cfg.max_gap + 1, im_w); ++left) {
-      hits.clear();
-      for (int j : table[left])
-        if (compatible(j, i)) hits.push_back(j);
-      if (!hits.empty()) return;
-    }
-    hits.clear();
-  };
-  auto precursors = [&](int i) {
-    const int x = (int)tp[i].x1;
-    const int lo = std::max((int)(tp[i].x1 - (float)cfg.max_gap), 0);
-    for (int left = x - 1; left >= lo; --left) {
-      hits.clear();
-      for (int j : table[left])
-        if (compatible(j, i)) hits.push_back(j);
-      if (!hits.empty()) return;
-    }
-    hits.clear();
-  };
+  // column table boxes_table[int(x1)] (graph_builder.py:62-64): a counting sort, ascending index within a column
+  std::vector<int> col_start(im_w + 1, 0), col_idx(m);
+  for (int i = 0; i < m; ++i) ++col_start[(int)tp[i].x1 + 1];
+  for (int c = 0; c < im_w; ++c) col_start[c + 1] += col_start[c];
+  std::vector<int> fill(col_start.begin(), col_start.end() - 1);
+  for (int i = 0; i < m; ++i) col_idx[fill[(int)tp[i].x1]++] = i;
   next.assign(m, -1);
   has_in.assign(m, 0);
   for (int i = 0; i < m; ++i) {
-    successions(i);
-    if (hits.empty()) continue;
-    int s = hits[0];
-    for (int j : hits)
-      if (sc[j] > sc[s]) s = j;          // np.argmax: first maximum
-    precursors(s);
-    float best = -INFINITY;
-    for (int j : hits) best = std::max(best, sc[j]);
-    if (!hits.empty() && sc[i] >= best) {  // is_succession_node
+    const int s = tl::successor(i, tp.data(), sc.data(), col_start.data(), col_idx.data(), im_w, cfg);
+    if (s >= 0) {
       next[i] = s;
       has_in[s] = 1;
     }
   }
   return CTPN_OK;
 }
-
 
 }  // namespace
 }  // namespace ctpn
@@ -302,58 +153,11 @@ extern "C" int ctpn_text_lines_host(const float *proposals, const float *scores,
   if (rc) return rc;
   // ---- chains (other.py:16-29) and lines ----
   std::vector<double> recs;   // 9 doubles per line
-  std::vector<float> X, Yt, Yb, S, Hh, Xc, Yc;
   for (int i = 0; i < m; ++i) {
     if (has_in[i] || next[i] < 0) continue;
-    X.clear(); Yt.clear(); Yb.clear(); S.clear(); Hh.clear(); Xc.clear(); Yc.clear();
-    float x0 = INFINITY, x1 = -INFINITY;
-    const int first = i;
-    int guard = 0;
-    for (int v = i; v >= 0 && guard <= m; v = next[v], ++guard) {
-      X.push_back(tp[v].x1); Yt.push_back(tp[v].y1); Yb.push_back(tp[v].y2); S.push_back(sc[v]);
-      Hh.push_back(tp[v].y2 - tp[v].y1);
-      Xc.push_back((tp[v].x1 + tp[v].x2) / 2.0f);
-      Yc.push_back((tp[v].y1 + tp[v].y2) / 2.0f);
-      x0 = std::min(x0, tp[v].x1);
-      x1 = std::max(x1, tp[v].x2);
-    }
-    const float off = (tp[first].x2 - tp[first].x1) * 0.5f;
-    double lt, rt, lb, rb;
-    fit_y(X, Yt, x0 + off, x1 - off, lt, rt);
-    fit_y(X, Yb, x0 + off, x1 - off, lb, rb);
-    const float score = np_sum_f32(S) / (float)S.size();
+    const tl::Chain chain{tp.data(), sc.data(), next.data(), i, tl::chain_length(next.data(), i, m)};
     double r[9];
-    if (!oriented) {
-      // text_proposal_connector.py:47-64 + clip_boxes (other.py:7-13: even columns incl. the score to [0, w-1])
-      float l0 = x0, l1 = (float)std::min(lt, rt), l2 = x1, l3 = (float)std::max(lb, rb), l4 = score;
-      const float wx = (float)(im_w - 1), hy = (float)(im_h - 1);
-      l0 = std::max(std::min(l0, wx), 0.f); l2 = std::max(std::min(l2, wx), 0.f); l4 = std::max(std::min(l4, wx), 0.f);
-      l1 = std::max(std::min(l1, hy), 0.f); l3 = std::max(std::min(l3, hy), 0.f);
-      r[0] = l0; r[1] = l1; r[2] = l2; r[3] = l1; r[4] = l0; r[5] = l3; r[6] = l2; r[7] = l3; r[8] = l4;
-    } else {
-      // text_proposal_connector_oriented.py:36-105
-      double z0d, z1d;
-      polyfit1(Xc, Yc, z0d, z1d);
-      const float z0 = (float)z0d, z1 = (float)z1d;
-      const float height = np_sum_f32(Hh) / (float)Hh.size() + 2.5f;
-      const float l0 = x0, l2 = x1, l5 = z0, l6 = z1, l7 = height;
-      const float b1 = l6 - l7 / 2.0f, b2 = l6 + l7 / 2.0f;
-      float px1 = l0, py1 = l5 * l0 + b1, px2 = l2, py2 = l5 * l2 + b1;
-      float px3 = l0, py3 = l5 * l0 + b2, px4 = l2, py4 = l5 * l2 + b2;
-      const float dx = px2 - px1, dy = py2 - py1;
-      const float width = std::sqrt(dx * dx + dy * dy);
-      const float t0 = py3 - py1;
-      const float t1 = t0 * dy / width;
-      const float ax = std::fabs(t1 * dx / width), ay = std::fabs(t1 * dy / width);
-      if (l5 < 0.f) { px1 -= ax; py1 += ay; px4 += ax; py4 -= ay; }
-      else { px2 += ax; py2 += ay; px3 -= ax; py3 -= ay; }
-      r[0] = px1; r[1] = py1; r[2] = px2; r[3] = py2; r[4] = px3; r[5] = py3; r[6] = px4; r[7] = py4; r[8] = score;
-    }
-    // filter_boxes (detectors.py:37-49), float64
-    const double h = (std::fabs(r[5] - r[1]) + std::fabs(r[7] - r[3])) / 2.0 + 1.0;
-    const double w = (std::fabs(r[2] - r[0]) + std::fabs(r[6] - r[4])) / 2.0 + 1.0;
-    if (w / h > cfg.min_ratio && r[8] > cfg.line_min_score && w > (double)(cfg.proposal_width * cfg.min_num_proposals))
-      recs.insert(recs.end(), r, r + 9);
+    if (tl::chain_line(chain, im_h, im_w, oriented, cfg, r)) recs.insert(recs.end(), r, r + 9);
   }
   const int L = (int)(recs.size() / 9);
   *num_lines = L;

@@ -8,6 +8,8 @@ and the annotated image.  `sess` is a ctpn_b200.Session (replaces tf.Session + S
 --batch N > 1 runs N images at a time through Engine.rois_ragged (images of different sizes in one batch), with the same
 resize, blob, TextDetector and output files per image (ctpn_batch).  --device-frontend (with --batch N) runs the resize
 and the blob on the GPU as well (Engine.rois_images, ctpn_batch_device); the output files are the same.
+--device-lines (with --device-frontend) builds the text lines on the GPU too (Engine.detect_lines_images): the files equal
+those of --device-frontend --native-connector.
 """
 from __future__ import print_function
 
@@ -30,10 +32,11 @@ from lib.fast_rcnn.config import cfg, cfg_from_file     # noqa: E402
 from lib.fast_rcnn.test import _get_image_blob, test_ctpn  # noqa: E402
 from lib.utils.timer import Timer                        # noqa: E402
 from lib.text_connector.detectors import TextDetector   # noqa: E402
-from lib.text_connector.text_connect_cfg import Config as TextLineCfg  # noqa: E402
+from lib.text_connector.text_connect_cfg import Config as TextLineCfg, native_cfg  # noqa: E402
 
 RESULTS_DIR = "data/results"
 NATIVE_CONNECTOR = False      # --native-connector: C++ text-line connector of the library instead of the Python one
+DEVICE_LINES = False          # --device-lines: the library's device connector on each batch's rois (Engine.detect_lines_images)
 
 
 def resize_im(im, scale, max_scale=None):
@@ -106,6 +109,15 @@ def ctpn_batch_device(sess, image_names):
     timer = Timer()
     timer.tic()
     imgs = [cv2.imread(name) for name in image_names]
+    if DEVICE_LINES:        # the lines of TextDetector(native=True), built on the device; only they come back with the images
+        res = sess.engine.detect_lines_images(imgs, mode=cfg.TEST.DETECT_MODE, return_resized=True, scale=TextLineCfg.SCALE,
+                                              max_scale=TextLineCfg.MAX_SCALE, cfg=native_cfg())
+        for name, (boxes, scale, img) in zip(image_names, res):
+            draw_boxes(img, name, boxes, scale)
+            print('{:s}: {:d} text lines'.format(name, boxes.shape[0]))
+        timer.toc()
+        print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
+        return
     res = sess.engine.rois_images(imgs, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
     for name, (r, im_scale, scale, img) in zip(image_names, res):
         scores, boxes = r[:, 0], r[:, 1:5] / np.float64(im_scale)      # the float64 division of test_ctpn
@@ -132,11 +144,17 @@ def main(argv=None):
     ap.add_argument("--device-frontend", action="store_true",
                     help="with --batch N: run resize_im and the image blob on the GPU (Engine.rois_images) instead of cv2 on "
                          "the host; same output files")
+    ap.add_argument("--device-lines", action="store_true",
+                    help="with --device-frontend: build the text lines on the GPU as well (Engine.detect_lines_images); same "
+                         "output files as --native-connector")
     args = ap.parse_args(argv)
     if args.device_frontend and args.batch <= 1:
         ap.error("--device-frontend needs --batch N with N > 1")
-    global NATIVE_CONNECTOR
+    if args.device_lines and not args.device_frontend:
+        ap.error("--device-lines needs --device-frontend (and --batch N with N > 1)")
+    global NATIVE_CONNECTOR, DEVICE_LINES
     NATIVE_CONNECTOR = args.native_connector
+    DEVICE_LINES = args.device_lines
     if os.path.exists(RESULTS_DIR):
         shutil.rmtree(RESULTS_DIR)
     os.makedirs(RESULTS_DIR)

@@ -45,6 +45,8 @@ SIGNATURES = {
     "ctpn_crc32c_host": (C.c_uint32, [_p, _z, C.c_uint32]),
     "ctpn_nms_host": (_i, [_p, _p, _p, _i, _i, _f, _i]),
     "ctpn_text_lines_host": (_i, [_p, _p, _i, _i, _i, _i, _p, _p, _i, _p]),
+    "ctpn_text_lines_workspace_bytes": (_z, [_i, _i, _i]),
+    "ctpn_text_lines": (_i, [_p, _p, _i, _i, _p, _p, _i, _p, _p, _p, _p, _p, _z, _p]),
     "ctpn_text_filter_nms_host": (_i, [_p, _p, _i, _p, _p, _p]),
     "ctpn_text_groups_host": (_i, [_p, _p, _i, _i, _p, _p, _p, _i, _p, _p]),
     "ctpn_bbox_overlaps_host": (_i, [_p, _i, _i, _p, _i, _i, _p]),

@@ -8,6 +8,7 @@ compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
     results = eng.detect_batch(uint8_batch)      # [B,H,W,3] -> list of (scores, boxes)
     results = eng.detect_ragged([im0, im1, ...])  # images of different sizes, batched on shared canvases
     results = eng.detect_images([photo0, ...])   # raw photos: resize_im + _get_image_blob on the device, then as above
+    lines = eng.detect_lines_images([photo0, ...])  # ... and the text-line connector on the device: ctpn() per image
 
 `planes` / `mode` select the arithmetic of the tensor-core layers (see include/ctpn_b200.h); accumulation is always
 float32:  1 / "bf16" = bf16 operands (1 unit per MAC);  2 / "bf16x2" = bf16x2 split, ~16 mantissa bits (3 units);
@@ -634,12 +635,23 @@ class Engine:
         resize_im output as a host uint8 array as a 4th item with return_resized (what draw_boxes draws on).  Every image
         is bit-identical to the host front-end with OpenCV's own code (IPP-dispatching cv2 builds differ on float
         rescales) followed by detect on that image alone.  Raises ValueError on a bad image (see frontend_plan)."""
-        if not 1 <= int(max_batch) <= 64:
-            raise ValueError("rois_images: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)")
-        images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
-        plan = frontend_plan(images, resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg)
         out = [None] * len(images)
         rows = self.result_rows()
+        for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
+                                                                "rois_images"):
+            for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, len(idxs), rows))):
+                out[i] = (r, items[k].im_scale, items[k].f) + ((resized[k],) if return_resized else ())
+        return out
+
+    def _images_batches(self, images, resize, max_batch, return_resized, scale, max_scale, what, after=None):
+        """The batches of rois_images / detect_lines_images.  Per ragged batch: front-end, network and proposal layer on the
+        device (detect_packed's buffer), then after(packed, items) -- device work enqueued on the rois, returning the buffer
+        to bring back (None: the packed rois themselves) -- and one D2H of that buffer.  Yields (input indices, their
+        FrontendSteps, the pinned host copy, the resize_im outputs or None); the pinned copy is reused by the next batch."""
+        if not 1 <= int(max_batch) <= 64:
+            raise ValueError("%s: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)" % what)
+        images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
+        plan = frontend_plan(images, resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg)
         lut = self._mean_lut()
         stream = N.stream_ptr()
         for idxs, (H, W) in ragged_plan([p.blob for p in plan], [p.dtype for p in plan], max_batch):
@@ -679,12 +691,102 @@ class Engine:
             info_h = self._pin("info", (B, 3), torch.float32)
             info_h.numpy()[...] = [[p.blob[0], p.blob[1], p.im_scale] for p in items]
             packed = self.detect_packed(canvas, info_h.to(self.device, non_blocking=True), sizes=np.array([p.blob for p in items]))
-            out_h = self._pin("out", tuple(packed.shape), torch.float32)
-            out_h.copy_(packed, non_blocking=True)
+            result = packed if after is None else after(packed, items)
+            out_h = self._pin("out", tuple(result.shape), result.dtype)
+            out_h.copy_(result, non_blocking=True)
             resized = [u8[k, :p.resized[0], :p.resized[1]].cpu().numpy() for k, p in enumerate(items)] if return_resized else None
             torch.cuda.current_stream().synchronize()              # also frees the pinned sources for the next batch
-            for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, B, rows))):
-                out[i] = (r, plan[i].im_scale, plan[i].f) + ((resized[k],) if return_resized else ())
+            yield idxs, items, out_h, resized
+
+    # ---- text lines on the device ----------------------------------------------------------
+    @staticmethod
+    def unpack_lines(packed, B, rows):
+        """Views (lines [B,rows,9] f64, num [B] i32, status [B] i32) of a packed text-line buffer [B*rows*9 + B] float64
+        (torch or numpy): the lines of all images followed by the int32 line counts and statuses (bit pattern)."""
+        n = B * rows * 9
+        lines = packed[:n].reshape(B, rows, 9)
+        tail = packed[n:]
+        t = tail.view(torch.int32) if torch.is_tensor(tail) else tail.view(np.int32)
+        return lines, t[:B], t[B:2 * B]
+
+    def text_lines(self, rois, count, im_hw, im_scales, mode="H", cfg=None, out=None, ws_key="lines"):
+        """TextDetector.detect for a batch on the device (ctpn_text_lines).  rois [B,rows,5] float32 and count [B] int32:
+        the proposal layer's output on this device (blob coordinates, rows in any order); im_hw [B,2] the (h, w) frame of
+        the lines (resize_im's output size) and im_scales [B] the blob scales, on the host.  mode "H" (axis-aligned, clipped)
+        or "O" (oriented); cfg: the 9 connector constants (see textlines.DEFAULT_CFG; None = those defaults).  Returns device
+        tensors (lines [B,rows,9] float64, num [B] int32, status [B] int32) without synchronising; for each image the first
+        num[b] rows equal textlines.text_lines(rois[b, :count[b], 1:5] / np.float64(im_scales[b]), rois[b, :count[b], 0],
+        im_hw[b], mode, cfg) bit for bit, and status[b] != 0 where that call would raise (see split_lines).
+        out=(lines, num, status): write into these contiguous tensors (e.g. views of a packed buffer, unpack_lines)."""
+        if mode not in ("H", "O"):
+            raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
+        assert rois.is_cuda and rois.dtype == torch.float32 and rois.dim() == 3 and rois.shape[2] == 5
+        assert count.is_cuda and count.dtype == torch.int32 and count.shape == (rois.shape[0],)
+        B, rows = int(rois.shape[0]), int(rois.shape[1])
+        hw = np.ascontiguousarray(np.asarray(im_hw, np.int64).reshape(-1, 2).astype(np.int32))
+        sc = np.ascontiguousarray(np.asarray(im_scales, np.float64).reshape(-1))
+        if hw.shape[0] != B or sc.shape[0] != B:
+            raise ValueError("text_lines: %d images but %d sizes and %d scales" % (B, hw.shape[0], sc.shape[0]))
+        cfg9 = None if cfg is None else np.ascontiguousarray(cfg, np.float32).reshape(9)
+        need = N.lib.ctpn_text_lines_workspace_bytes(B, rows, max(1, int(hw[:, 1].max())))
+        ws = self._workspace(ws_key, need)
+        if out is not None:
+            lines, num, status = out
+            assert lines.shape == (B, rows, 9) and lines.dtype == torch.float64 and num.shape == status.shape == (B,)
+            assert lines.is_contiguous() and num.is_contiguous() and status.is_contiguous()
+        else:
+            lines = torch.empty((B, rows, 9), dtype=torch.float64, device=self.device)
+            num = torch.empty((B,), dtype=torch.int32, device=self.device)
+            status = torch.empty((B,), dtype=torch.int32, device=self.device)
+        N.check(N.lib.ctpn_text_lines(N.ptr(rois.contiguous()), N.ptr(count.contiguous()), B, rows, N.ptr(hw), N.ptr(sc), 1 if mode == "O" else 0,
+                                      N.ptr(cfg9), N.ptr(lines), N.ptr(num), N.ptr(status), N.ptr(ws), ws.numel(), N.stream_ptr()),
+                "ctpn_text_lines")
+        return lines, num, status
+
+    @staticmethod
+    def split_lines(lines, num, status, im_hw=None):
+        """Host copies of text_lines' results -> one float64 [num[b], 9] array per image.  Raises CtpnError for an image
+        whose status is nonzero, as the host connector raises on it (status 1: a proposal's x1 outside the image width,
+        where the reference raises IndexError; 2: a count outside [0, rows])."""
+        lines, num, status = (t.cpu().numpy() if torch.is_tensor(t) else np.asarray(t) for t in (lines, num, status))
+        out = []
+        for b in range(lines.shape[0]):
+            st = int(status[b])
+            if st == 1:
+                width = "" if im_hw is None else " %d" % int(np.asarray(im_hw).reshape(-1, 2)[b, 1])
+                raise N.CtpnError("text lines of image %d: a proposal's x1 lies outside the image width%s" % (b, width))
+            if st:
+                raise N.CtpnError("text lines of image %d: status %d (proposal count outside [0, rows])" % (b, st))
+            out.append(lines[b, :int(num[b])].copy())
+        return out
+
+    def detect_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
+                            cfg=None):
+        """ctpn() (demo.py:55-68 minus file I/O) for a list of raw HxWx3 uint8 BGR images of any sizes, all on the device:
+        the batches of rois_images (same inputs and batching), then the text-line connector (text_lines) on each batch's
+        rois, and one D2H per batch of the packed lines, counts and statuses.  Returns, in input order, (lines float64
+        [m,9] (x1,y1,x2,y2,x3,y3,x4,y4,score) in the resize_im frame, f) per image, plus the resize_im output with
+        return_resized.  lines is bit-identical to TextDetector(native=True).detect(boxes, scores[:, None], resized.shape[:2])
+        on detect_images' output for that image (mode "H" / "O" as cfg.TEST.DETECT_MODE; cfg: the 9 connector constants,
+        None = text_connect_cfg's).  Raises CtpnError where that connector raises (a proposal outside the image width)."""
+        if mode not in ("H", "O"):
+            raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
+        rows = self.result_rows()
+
+        def connect(packed, items):
+            B = len(items)
+            rois, count = self.unpack(packed, B, rows)
+            res = torch.empty(B * rows * 9 + B, dtype=torch.float64, device=self.device)
+            self.text_lines(rois, count, [p.resized for p in items], [p.im_scale for p in items], mode, cfg,
+                            out=self.unpack_lines(res, B, rows))
+            return res
+
+        out = [None] * len(images)
+        for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
+                                                                "detect_lines_images", after=connect):
+            per_image = self.split_lines(*self.unpack_lines(out_h.numpy(), len(idxs), rows), im_hw=[p.resized for p in items])
+            for k, (i, lines) in enumerate(zip(idxs, per_image)):
+                out[i] = (lines, items[k].f) + ((resized[k],) if return_resized else ())
         return out
 
     def detect_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200):
