@@ -513,3 +513,12 @@ extern "C" int ctpn_net_debug_tap(ctpn_net_t *net, const char *name, float *out_
   }
   return CTPN_OK;
 }
+
+#ifdef CTPN_DEBUG
+extern "C" int ctpn_net_f16f8_scales(const ctpn_net_t *net, float *s, float *t, float *amax) {
+  CTPN_REQUIRE(net && s && t && amax, "ctpn_net_f16f8_scales: null pointer");
+  CTPN_REQUIRE(net->f16f8 && net->calibrated, "ctpn_net_f16f8_scales: not a calibrated F16F8 net");
+  for (int l = 0; l < 13; ++l) { s[l] = net->act_s[l]; t[l] = net->act_t[l]; amax[l] = net->act_max[l]; }
+  return CTPN_OK;
+}
+#endif

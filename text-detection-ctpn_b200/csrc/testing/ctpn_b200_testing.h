@@ -28,6 +28,11 @@ int ctpn_conv3x3_simt(const void *in_planes, const void *w_planes, const float *
                       int B, int H, int W, int cin, int cout, int taps, int planes, int flags,
                       void *stream);
 
+/* The activation scales a calibrated F16F8 net (CTPN_ARITH_F16F8) derived for the outputs of conv1_1 .. conv5_3: s[13],
+ * t[13] and the calibration maximum amax[13] from which they were derived (net.cu::calibrate_f16f8).  CTPN_ERR_INVALID
+ * before the first forward or on another arithmetic. */
+int ctpn_net_f16f8_scales(const ctpn_net_t *net, float *s, float *t, float *amax);
+
 
 /* ---- hardware probes ---------------------------------------------------------------------
  * Hardware probe used by tests/probe_umma_view.py: reads a [rows][64] bf16 matrix through a wgmma

@@ -85,6 +85,7 @@ TESTING_SIGNATURES = {
     "ctpn_conv1_1": (_i, [_p, _i, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
     "ctpn_conv3x3_simt": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _p]),
     "ctpn_probe_umma_view": (_i, [_p, _p, _i, _i, _i, _i, _p, _p]),
+    "ctpn_net_f16f8_scales": (_i, [_p, _p, _p, _p]),
 }
 
 for _name, (_res, _args) in list(SIGNATURES.items()) + (list(TESTING_SIGNATURES.items()) if DEBUG_LIB else []):

@@ -148,8 +148,10 @@ class Engine:
     def recalibrate(self):
         """F16F8 mode: derive the activation scales again from the next batch (they are frozen after the first one).
         The scales put each layer's calibration maximum two binades below e4m3 saturation; activations beyond that saturate
-        in the e4m3 copies only (those elements fall back to fp16 accuracy), so calibrate on representative images -- not on
-        a flat warm-up image -- and call this again when the input distribution changes."""
+        in the e4m3 copies, and those elements fall back to fp16 accuracy as long as they stay below 65504 / s in the fp16
+        plane.  s is 1 unless the calibration maximum exceeds 2^14; a layer with s < 1 has only 2-3 binades of fp16 headroom,
+        past which the element saturates in fp16 too and its error is unbounded.  So calibrate on representative images --
+        not on a flat warm-up image -- and call this again when the input distribution changes."""
         N.check(N.lib.ctpn_net_set_option(self._net, b"recalibrate", 1), "set_option")
         self._graphs.clear()          # captured graphs hold the old scales as kernel arguments
 
