@@ -22,6 +22,7 @@
  *   ctpn_resize_linear_u8   cv2.resize in resize_im, ctpn/demo.py:21-25 (and draw_boxes :50)
  *   ctpn_image_blob_f32     _get_image_blob, lib/fast_rcnn/test.py:7-31 (float32 cv2.resize of the mean-subtracted image)
  *   ctpn_resize_linear_u8_ragged / ctpn_image_blob_f32_ragged   the same two, for a batch of images of different sizes
+ *   ctpn_resize_linear_u8_ragged_rows     the ragged resize on sources that hold only the rows it reads
  *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host / ctpn_text_lines (batched, device)
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
@@ -237,6 +238,24 @@ int ctpn_resize_linear_u8_ragged(const void *src, size_t src_elems, const long l
 int ctpn_image_blob_f32_ragged(const void *src_u8, size_t src_elems, const long long *src_offset, const int *src_hwp,
                                const double *fxy, const int *dst_hw, const float *lut, int B, float *dst, int H, int W,
                                void *stream);
+
+/* ctpn_resize_linear_u8_ragged for row-compacted sources: INTER_LINEAR reads two source rows per output row, so a strong
+ * downscale (f = 0.2: 2 of every 5 rows) leaves most rows unread, and a caller that uploads the images need not send
+ * them.  Image b is [stored_rows[b]][pitch][C] at src + src_offset[b]: a subset of the rows of the (h, w) = src_hwp image,
+ * in ascending order, holding at least every row the resize reads.  row_map (DEVICE int32, map_elems entries) holds, at
+ * map_offset[b], one entry per ORIGINAL row y < h: the stored index of row y (any value for rows that are not stored;
+ * the identity for an image stored densely, which an exact 1/2 scale must be: its INTER_AREA route reads every row).
+ * Taps, weights, border clamping and the output size come from the original (h, w) exactly as in the dense call -- the
+ * same per-pixel code -- and only the row address goes through the map, so with a correct map every image is bit-identical
+ * to ctpn_resize_linear_u8_ragged on the full image.  stored_rows and map_offset are HOST arrays like the other
+ * descriptors.  Validated before any CUDA call, in addition to the dense call's checks (CTPN_ERR_INVALID naming the
+ * image): 1 <= stored_rows <= h, offset + ((stored_rows - 1) * pitch + w) * C <= src_elems, map_offset >= 0 and
+ * map_offset + h <= map_elems.  The map's CONTENT is not trusted: the kernel clamps every entry to [0, stored_rows), so
+ * a wrong map gives wrong pixels, never a read outside the extent that was checked. */
+int ctpn_resize_linear_u8_ragged_rows(const void *src, size_t src_elems, const long long *src_offset, const int *src_hwp,
+                                      const int *stored_rows, const int *row_map, size_t map_elems, const long long *map_offset,
+                                      const double *fxy, const int *dst_hw, int B, int channels, void *dst, int H, int W,
+                                      void *stream);
 
 /* CRC-32C (Castagnoli) of a host buffer, continuing from `crc` (0 to start): the per-tensor checksum of TF checkpoint V2
  * files, used by the weight importer (ctpn_b200/tf_import.py) to verify every tensor it loads. */

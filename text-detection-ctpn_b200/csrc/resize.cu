@@ -18,7 +18,8 @@
 // for float images; this kernel is bit-exact with the open implementation.
 //
 // The *_ragged entry points run both for a batch of images of different sizes (Engine.rois_images); they share the
-// per-pixel functions below with the single-image kernels.
+// per-pixel functions below with the single-image kernels.  ctpn_resize_linear_u8_ragged_rows is the ragged resize on
+// sources that hold only the rows it reads (Engine.stream_rois_images uploads camera photos that way).
 #include "common.cuh"
 
 namespace ctpn {
@@ -38,17 +39,33 @@ __device__ __forceinline__ void resize_taps(int d, int sn, double scale, bool dr
   s1 = min(max(s + 1, 0), sn - 1);
 }
 
+// Where source row y of an image is stored: every row in place ...
+struct DenseRows {
+  __device__ __forceinline__ int operator()(int y) const { return y; }
+};
+// ... or only the rows the resize reads (ctpn_resize_linear_u8_ragged_rows): map[y] is the stored index of source row y.
+// The map is device memory the host never saw, so the index is clamped to the stored extent the host did check.
+struct CompactRows {
+  const int *__restrict__ map;
+  int stored;
+  __device__ __forceinline__ int operator()(int y) const { return min(max(__ldg(map + y), 0), stored - 1); }
+};
+
 // One output pixel of cv2.resize(INTER_LINEAR) of a uint8 image im [sh][pitch][C] (pitch >= sw pixels per row) -> o[C].
-// Shared by the uniform and the ragged kernel: the ragged batch is bit-identical to single-image runs by construction.
+// Shared by the uniform and the ragged kernels: the ragged batch is bit-identical to single-image runs by construction.
+// Taps, weights and border clamping come from the source geometry (sh, sw); only the address of a row goes through
+// `row`.
+template <class Rows>
 __device__ __forceinline__ void resize_u8_pixel(const uint8_t *__restrict__ im, int sh, int sw, int pitch, int C, int dx, int dy,
-                                                double scale_x, double scale_y, bool area2, uint8_t *__restrict__ o) {
+                                                double scale_x, double scale_y, bool area2, uint8_t *__restrict__ o,
+                                                const Rows row) {
   if (area2) {
     const int y0 = 2 * dy, x0 = 2 * dx;
     const int ny = min(2, sh - y0), nx = min(2, sw - x0);
     for (int c = 0; c < C; ++c) {
       int sum = 0;
       for (int yy = 0; yy < ny; ++yy)
-        for (int xx = 0; xx < nx; ++xx) sum += im[((size_t)(y0 + yy) * pitch + x0 + xx) * C + c];
+        for (int xx = 0; xx < nx; ++xx) sum += im[((size_t)row(y0 + yy) * pitch + x0 + xx) * C + c];
       int v = (ny * nx == 4) ? (sum + 2) >> 2 : __float2int_rn(__fdiv_rn((float)sum, (float)(ny * nx)));
       o[c] = (uint8_t)min(max(v, 0), 255);
     }
@@ -57,7 +74,7 @@ __device__ __forceinline__ void resize_u8_pixel(const uint8_t *__restrict__ im, 
   int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
   resize_taps(dx, sw, scale_x, true, sx0, sx1, a0, a1);
   resize_taps(dy, sh, scale_y, false, sy0, sy1, b0, b1);
-  const uint8_t *r0 = im + (size_t)sy0 * pitch * C, *r1 = im + (size_t)sy1 * pitch * C;
+  const uint8_t *r0 = im + (size_t)row(sy0) * pitch * C, *r1 = im + (size_t)row(sy1) * pitch * C;
   for (int c = 0; c < C; ++c) {
     const int h0 = r0[(size_t)sx0 * C + c] * a0 + r0[(size_t)sx1 * C + c] * a1;
     const int h1 = r1[(size_t)sx0 * C + c] * a0 + r1[(size_t)sx1 * C + c] * a1;
@@ -72,7 +89,8 @@ resize_linear_u8_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ d
   const long long total = (long long)B * dh * dw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int dx = (int)(i % dw), dy = (int)((i / dw) % dh), b = (int)(i / ((long long)dw * dh));
-    resize_u8_pixel(src + (size_t)b * sh * sw * C, sh, sw, sw, C, dx, dy, scale_x, scale_y, area2 != 0, dst + (size_t)i * C);
+    resize_u8_pixel(src + (size_t)b * sh * sw * C, sh, sw, sw, C, dx, dy, scale_x, scale_y, area2 != 0, dst + (size_t)i * C,
+                    DenseRows());
   }
 }
 
@@ -157,7 +175,31 @@ __global__ void __launch_bounds__(256) resize_linear_u8_ragged_kernel(const uint
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int dx = (int)(i % dw), dy = (int)(i / dw);
     resize_u8_pixel(im, p.sh[b], p.sw[b], p.pitch[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
-                    out + ((size_t)dy * p.W + dx) * C);
+                    out + ((size_t)dy * p.W + dx) * C, DenseRows());
+  }
+}
+
+// Row-compacted sources: image b stores only stored[b] of its sh[b] rows, and rows + map_offset[b] is its row map
+// (sh[b] entries, see CompactRows).  Same launch shape and per-pixel code as the kernel above.
+struct RaggedResizeRows {
+  RaggedResize r;
+  long long map_offset[kRaggedMax];
+  int stored[kRaggedMax];
+};
+
+__global__ void __launch_bounds__(256) resize_linear_u8_ragged_rows_kernel(const uint8_t *__restrict__ src,
+                                                                           const int *__restrict__ rows, uint8_t *__restrict__ dst,
+                                                                           const __grid_constant__ RaggedResizeRows q) {
+  const RaggedResize &p = q.r;
+  const int b = blockIdx.y, dh = p.dh[b], dw = p.dw[b], C = p.C;
+  const uint8_t *im = src + p.src_offset[b];
+  const CompactRows row{rows + q.map_offset[b], q.stored[b]};
+  uint8_t *out = dst + (size_t)b * p.H * p.W * C;
+  const long long total = (long long)dh * dw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int dx = (int)(i % dw), dy = (int)(i / dw);
+    resize_u8_pixel(im, p.sh[b], p.sw[b], p.pitch[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
+                    out + ((size_t)dy * p.W + dx) * C, row);
   }
 }
 
@@ -231,8 +273,10 @@ extern "C" int ctpn_image_blob_f32(const void *src_u8, const float *lut, int B, 
 }
 
 // Validates the per-image host descriptors of a ragged call and fills the kernel's parameter struct; no CUDA call.
+// stored (NULL: every row): how many of image b's rows the source holds (row-compacted sources).
 static int ragged_params(const char *fn, size_t src_elems, const long long *src_offset, const int *src_hwp, const double *fxy,
-                         const int *dst_hw, int B, int C, int H, int W, RaggedResize *p, long long *max_pixels) {
+                         const int *dst_hw, int B, int C, int H, int W, RaggedResize *p, long long *max_pixels,
+                         const int *stored = nullptr) {
   CTPN_REQUIRE(src_offset && src_hwp && fxy && dst_hw, "%s: null descriptor array", fn);
   CTPN_REQUIRE(B >= 1 && B <= kRaggedMax, "%s: B = %d, must be 1..%d", fn, B, kRaggedMax);
   CTPN_REQUIRE(H > 0 && W > 0, "%s: bad canvas %d x %d", fn, H, W);
@@ -250,8 +294,10 @@ static int ragged_params(const char *fn, size_t src_elems, const long long *src_
     CTPN_REQUIRE(fx > 0 && fy > 0, "%s: image %d: scale (%g, %g) must be > 0", fn, b, fx, fy);
     CTPN_REQUIRE(sh * fy < 1e9 && sw * fx < 1e9, "%s: image %d: scale (%g, %g) too large", fn, b, fx, fy);
     CTPN_REQUIRE(off >= 0, "%s: image %d: negative source offset %lld", fn, b, off);
+    const int held = stored ? stored[b] : sh;
+    CTPN_REQUIRE(held >= 1 && held <= sh, "%s: image %d: %d stored rows, must be 1..%d (the source height)", fn, b, held, sh);
     const unsigned __int128 end = (unsigned __int128)off +
-                                  ((unsigned __int128)(sh - 1) * (unsigned)pitch + (unsigned)sw) * (unsigned)C;
+                                  ((unsigned __int128)(held - 1) * (unsigned)pitch + (unsigned)sw) * (unsigned)C;
     CTPN_REQUIRE(end <= (unsigned __int128)src_elems, "%s: image %d: source extent ends at %llu, past src_elems = %zu", fn, b,
                  (unsigned long long)end, src_elems);
     int eh = 0, ew = 0;
@@ -300,6 +346,36 @@ extern "C" int ctpn_resize_linear_u8_ragged(const void *src, size_t src_elems, c
   for (int b = 0; b < B; ++b) work += (long long)p.dh[b] * p.dw[b] * channels;
   ProfScope prof("resize_linear_u8_ragged", (double)work, (cudaStream_t)stream);
   resize_linear_u8_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src, (uint8_t *)dst, p);
+  CTPN_LAUNCH_CHECK();
+  return CTPN_OK;
+}
+
+extern "C" int ctpn_resize_linear_u8_ragged_rows(const void *src, size_t src_elems, const long long *src_offset, const int *src_hwp,
+                                                 const int *stored_rows, const int *row_map, size_t map_elems,
+                                                 const long long *map_offset, const double *fxy, const int *dst_hw, int B,
+                                                 int channels, void *dst, int H, int W, void *stream) {
+  const char *fn = "ctpn_resize_linear_u8_ragged_rows";
+  CTPN_REQUIRE(src && dst && row_map, "%s: null pointer", fn);
+  CTPN_REQUIRE(stored_rows && map_offset, "%s: null descriptor array", fn);
+  CTPN_REQUIRE(channels > 0 && channels <= 4, "%s: bad channel count %d", fn, channels);
+  RaggedResizeRows q;
+  long long max_pixels = 0, work = 0;
+  int rc = ragged_params(fn, src_elems, src_offset, src_hwp, fxy, dst_hw, B, channels, H, W, &q.r, &max_pixels, stored_rows);
+  if (rc) return rc;
+  memset(q.map_offset, 0, sizeof(q.map_offset));
+  memset(q.stored, 0, sizeof(q.stored));
+  for (int b = 0; b < B; ++b) {
+    const long long off = map_offset[b];
+    CTPN_REQUIRE(off >= 0 && (unsigned long long)off <= map_elems && (size_t)q.r.sh[b] <= map_elems - (size_t)off,
+                 "%s: image %d: row map [%lld, %lld + %d) lies outside map_elems = %zu", fn, b, off, off, q.r.sh[b], map_elems);
+    q.map_offset[b] = off;
+    q.stored[b] = stored_rows[b];
+  }
+  dim3 grid;
+  if ((rc = ragged_grid(B, max_pixels, &grid))) return rc;
+  for (int b = 0; b < B; ++b) work += (long long)q.r.dh[b] * q.r.dw[b] * channels;
+  ProfScope prof("resize_linear_u8_ragged_rows", (double)work, (cudaStream_t)stream);
+  resize_linear_u8_ragged_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src, row_map, (uint8_t *)dst, q);
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
 }

@@ -9,7 +9,9 @@ and the annotated image.  `sess` is a ctpn_b200.Session (replaces tf.Session + S
 resize, blob, TextDetector and output files per image (ctpn_batch).  --device-frontend (with --batch N) runs the resize
 and the blob on the GPU as well (Engine.rois_images, ctpn_batch_device); the output files are the same.
 --device-lines (with --device-frontend) builds the text lines on the GPU too (Engine.detect_lines_images): the files equal
-those of --device-frontend --native-connector.
+those of --device-frontend --native-connector.  --stream (with --device-frontend) reads and decodes the files one at a
+time while earlier ones are uploaded and computed (Engine.stream_rois_images / stream_lines_images, ctpn_stream_device);
+the output files are the same.
 """
 from __future__ import print_function
 
@@ -129,6 +131,31 @@ def ctpn_batch_device(sess, image_names):
     print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
 
 
+def ctpn_stream_device(sess, image_names, batch):
+    """ctpn_batch_device for the whole folder as one stream: every file is decoded when the pipeline asks for it
+    (Engine.stream_rois_images / stream_lines_images pull a window of images at a time), and each image's files are
+    written when its result arrives, while later images are still on their way."""
+    timer = Timer()
+    timer.tic()
+    decoded = (cv2.imread(name) for name in image_names)
+    kw = dict(max_batch=batch, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
+    if DEVICE_LINES:
+        results = sess.engine.stream_lines_images(decoded, mode=cfg.TEST.DETECT_MODE, cfg=native_cfg(), **kw)
+    else:
+        results = sess.engine.stream_rois_images(decoded, **kw)
+    for name, res in zip(image_names, results):
+        if DEVICE_LINES:
+            boxes, scale, img = res
+        else:
+            r, im_scale, scale, img = res
+            scores, boxes = r[:, 0], r[:, 1:5] / np.float64(im_scale)      # the float64 division of test_ctpn
+            boxes = TextDetector(native=NATIVE_CONNECTOR).detect(boxes, scores[:, np.newaxis], img.shape[:2])
+        draw_boxes(img, name, boxes, scale)
+        print('{:s}: {:d} text lines'.format(name, boxes.shape[0]))
+    timer.toc()
+    print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--weights", default=None,
@@ -147,7 +174,12 @@ def main(argv=None):
     ap.add_argument("--device-lines", action="store_true",
                     help="with --device-frontend: build the text lines on the GPU as well (Engine.detect_lines_images); same "
                          "output files as --native-connector")
+    ap.add_argument("--stream", action="store_true",
+                    help="with --device-frontend: decode the files lazily and overlap decoding, upload and compute "
+                         "(Engine.stream_rois_images / stream_lines_images); same output files")
     args = ap.parse_args(argv)
+    if args.stream and not args.device_frontend:
+        ap.error("--stream needs --device-frontend (and --batch N with N > 1)")
     if args.device_frontend and args.batch <= 1:
         ap.error("--device-frontend needs --batch N with N > 1")
     if args.device_lines and not args.device_frontend:
@@ -176,6 +208,10 @@ def main(argv=None):
     if args.planes == 4:                                # F16F8: take the activation scales from the first real image, not from the flat
         sess.engine.recalibrate()                       # grey warm-up image
     names = sorted(glob.glob(args.images))
+    if args.stream:
+        print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')
+        ctpn_stream_device(sess, names, args.batch)
+        return
     if args.batch > 1:
         for k in range(0, len(names), args.batch):
             print('~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~~')

@@ -9,6 +9,8 @@ compute is in libctpn_b200.so (see include/ctpn_b200.h).  One Engine == one GPU.
     results = eng.detect_ragged([im0, im1, ...])  # images of different sizes, batched on shared canvases
     results = eng.detect_images([photo0, ...])   # raw photos: resize_im + _get_image_blob on the device, then as above
     lines = eng.detect_lines_images([photo0, ...])  # ... and the text-line connector on the device: ctpn() per image
+    for scores, boxes, f in eng.stream_images(cv2.imread(p) for p in paths): ...   # the same from any iterable, in input
+                                                 # order, with packing, upload, compute and download overlapped
 
 `planes` / `mode` select the arithmetic of the tensor-core layers (see include/ctpn_b200.h); accumulation is always
 float32:  1 / "bf16" = bf16 operands (1 unit per MAC);  2 / "bf16x2" = bf16x2 split, ~16 mantissa bits (3 units);
@@ -110,23 +112,29 @@ class Engine:
         N.check(N.lib.ctpn_net_feature_hw(H, W, C.byref(fh), C.byref(fw)), "ctpn_net_feature_hw")
         return fh.value, fw.value
 
-    def _sizes_device(self, sizes, B, H, W, least=16, what="sizes"):
-        """Per-image (h, w) of a ragged batch on its [B, H, W] canvas -> device int32 [B,2], checked on the host."""
+    def _sizes_device(self, sizes, B, H, W, least=16, what="sizes", device=None):
+        """Per-image (h, w) of a ragged batch on its [B, H, W] canvas -> device int32 [B,2], checked on the host.
+        device: a device int32 [B,2] tensor that already holds (or, in stream order, will hold) these sizes -- returned
+        instead of uploading them, which costs a pageable copy and a stream synchronise per call."""
         s = sizes.cpu().numpy() if torch.is_tensor(sizes) else np.asarray(sizes)
         s = np.asarray(s, np.int64).reshape(-1, 2) if s.size else s.reshape(0, 2)
         if s.shape != (B, 2):
             raise ValueError("%s: expected %d (h, w) pairs, got shape %s" % (what, B, tuple(np.shape(sizes))))
         if (s[:, 0] > H).any() or (s[:, 1] > W).any() or (s < least).any():
             raise ValueError("%s: every (h, w) must lie within the %dx%d canvas and be at least %d" % (what, H, W, least))
+        if device is not None:
+            assert device.is_cuda and device.dtype == torch.int32 and tuple(device.shape) == (B, 2) and device.is_contiguous()
+            return device
         return torch.from_numpy(s.astype(np.int32)).to(self.device, non_blocking=False)
 
     # ---- stages ----------------------------------------------------------------------------
-    def forward_heads(self, images, ws_key="net", sizes=None):
+    def forward_heads(self, images, ws_key="net", sizes=None, sizes_device=None):
         """images: CUDA tensor [B,H,W,3], uint8 BGR (mean subtraction fused) or float32 blob
         (already mean-subtracted, test.py:9).  Returns (rpn_cls_score [B,h,w,20] logits,
         rpn_bbox_pred [B,h,w,40]) float32 CUDA tensors.
         sizes: [B,2] (h, w) per image for a ragged batch (image b in rows < h and columns < w of its canvas slice, the rest
-        ignored); each image's heads within (h >> 4, w >> 4) then equal a forward of that image alone.  None: uniform."""
+        ignored); each image's heads within (h >> 4, w >> 4) then equal a forward of that image alone.  None: uniform.
+        sizes_device: the same sizes already on the device (see _sizes_device)."""
         assert images.is_cuda and images.dim() == 4 and images.shape[3] == 3 and images.is_contiguous()
         is_f32 = images.dtype == torch.float32
         assert is_f32 or images.dtype == torch.uint8
@@ -140,7 +148,7 @@ class Engine:
             N.check(N.lib.ctpn_net_forward(self._net, N.ptr(images), int(is_f32), B, H, W, N.ptr(cls), N.ptr(bbox),
                                            N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward")
         else:
-            sz = self._sizes_device(sizes, B, H, W)
+            sz = self._sizes_device(sizes, B, H, W, device=sizes_device)
             N.check(N.lib.ctpn_net_forward_ragged(self._net, N.ptr(images), int(is_f32), N.ptr(sz), B, H, W, N.ptr(cls),
                                                   N.ptr(bbox), N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward_ragged")
         return cls, bbox
@@ -163,12 +171,14 @@ class Engine:
         N.check(N.lib.ctpn_net_debug_tap(self._net, name.encode(), N.ptr(out), out.numel(), C.byref(cnt), N.stream_ptr()), "debug_tap")
         return out
 
-    def proposals(self, cls, bbox, im_info, cls_is_logit=True, cfg=None, ws_key="prop", out=None, feat_sizes=None):
+    def proposals(self, cls, bbox, im_info, cls_is_logit=True, cfg=None, ws_key="prop", out=None, feat_sizes=None,
+                  feat_sizes_device=None):
         """Batched proposal layer (proposal_layer_tf.py:14-157) on CUDA tensors.
         Returns rois [B,post,5] (score,x1,y1,x2,y2), index [B,post] int32, count [B] int32.
         out=(rois, count): write into these (contiguous) tensors instead of allocating.
         feat_sizes: [B,2] (fh, fw) per image of a ragged batch: only those cells of each image's heads are read, and index is
-        image-local ((h * fw + w) * 10 + a).  None: every cell."""
+        image-local ((h * fw + w) * 10 + a).  None: every cell.  feat_sizes_device: feat_sizes already on the device (see
+        _sizes_device)."""
         c = dict(self.cfg)
         if cfg:
             c.update(cfg)
@@ -188,7 +198,7 @@ class Engine:
         index = torch.empty((B, rows), dtype=torch.int32, device=self.device)
         im_info = im_info.to(device=self.device, dtype=torch.float32).contiguous()
         if feat_sizes is not None:
-            fs = self._sizes_device(feat_sizes, B, H, W, least=1, what="feat_sizes")
+            fs = self._sizes_device(feat_sizes, B, H, W, least=1, what="feat_sizes", device=feat_sizes_device)
             N.check(N.lib.ctpn_proposals_ragged(N.ptr(cls.contiguous()), int(cls_is_logit), N.ptr(bbox.contiguous()), N.ptr(im_info),
                                                 N.ptr(fs), B, H, W, int(c["FEAT_STRIDE"]), pre, post, float(c["RPN_NMS_THRESH"]),
                                                 float(c["RPN_MIN_SIZE"]), int(bool(c["ANCHORS_PY2"])), N.ptr(rois), N.ptr(index),
@@ -217,12 +227,14 @@ class Engine:
         count = tail.view(torch.int32) if torch.is_tensor(tail) else tail.view(np.int32)
         return rois, count
 
-    def detect_packed(self, images, im_info, ws_tag="", sizes=None):
+    def detect_packed(self, images, im_info, ws_tag="", sizes=None, device_sizes=None):
         """images: CUDA [B,H,W,3] uint8/float32; im_info: [B,3] tensor (blob_h, blob_w, scale).
         Returns ONE float32 device buffer [B*post*5 + B]: the rois of all images followed by the int32 counts
         (bit pattern), so that the D2H / the multi-GPU gather of a batch's results is a single transfer.
-        sizes: [B,2] (h, w) per image of a ragged batch (see forward_heads), or None."""
+        sizes: [B,2] (h, w) per image of a ragged batch (see forward_heads), or None.  device_sizes: (sizes, sizes >> 4) as
+        device int32 [B,2] tensors, when the caller has uploaded them with the batch (see _sizes_device)."""
         B = int(images.shape[0])
+        sz_d, feat_d = device_sizes if device_sizes is not None else (None, None)
         if sizes is not None:
             sizes = np.asarray(sizes.cpu() if torch.is_tensor(sizes) else sizes, np.int64).reshape(-1, 2)
             feat = sizes >> 4
@@ -231,9 +243,9 @@ class Engine:
         rois, count = self.unpack(packed, B, rows)
         n = min(self.streams, B)
         if n <= 1:
-            cls, bbox = self.forward_heads(images, ws_key="net" + ws_tag, sizes=sizes)
+            cls, bbox = self.forward_heads(images, ws_key="net" + ws_tag, sizes=sizes, sizes_device=sz_d)
             self.proposals(cls, bbox, im_info, cls_is_logit=True, ws_key="prop" + ws_tag, out=(rois, count),
-                           feat_sizes=None if sizes is None else feat)
+                           feat_sizes=None if sizes is None else feat, feat_sizes_device=feat_d)
             return packed
         # sub-batches on side streams: the SIMT kernels of one sub-batch (conv1_1, BiLSTM, sort, NMS) run beside
         # the tensor-core kernels of the other (a persistent conv CTA leaves room for them on every SM)
@@ -247,9 +259,11 @@ class Engine:
             st.wait_stream(main)
             with torch.cuda.stream(st):
                 lo, hi = bounds[i], bounds[i + 1]
-                cls, bbox = self.forward_heads(images[lo:hi], ws_key="net%d" % i, sizes=None if sizes is None else sizes[lo:hi])
+                cls, bbox = self.forward_heads(images[lo:hi], ws_key="net%d" % i, sizes=None if sizes is None else sizes[lo:hi],
+                                               sizes_device=None if sz_d is None else sz_d[lo:hi])
                 self.proposals(cls, bbox, im_info[lo:hi], cls_is_logit=True, ws_key="prop%d" % i, out=(rois[lo:hi], count[lo:hi]),
-                               feat_sizes=None if sizes is None else feat[lo:hi])
+                               feat_sizes=None if sizes is None else feat[lo:hi],
+                               feat_sizes_device=None if feat_d is None else feat_d[lo:hi])
         for st in self._side[:n]:
             main.wait_stream(st)
         return packed
@@ -776,12 +790,7 @@ class Engine:
         rows = self.result_rows()
 
         def connect(packed, items):
-            B = len(items)
-            rois, count = self.unpack(packed, B, rows)
-            res = torch.empty(B * rows * 9 + B, dtype=torch.float64, device=self.device)
-            self.text_lines(rois, count, [p.resized for p in items], [p.im_scale for p in items], mode, cfg,
-                            out=self.unpack_lines(res, B, rows))
-            return res
+            return self._connect(packed, items, mode, cfg)
 
         out = [None] * len(images)
         for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
@@ -798,6 +807,211 @@ class Engine:
         res = self.rois_images(images, resize=resize, max_batch=max_batch, return_resized=return_resized, scale=scale,
                                max_scale=max_scale)
         return [(r[0][:, 0], r[0][:, 1:5] / np.float64(r[1])) + tuple(r[2:]) for r in res]
+
+    # ---- streamed photos: staging, upload and compute overlapped ---------------------------------
+    def _stream_buffer(self, kind, slot, nbytes, stream=None):
+        """Grow-only uint8 buffer `kind` of pipeline slot `slot`: pinned host memory for kind "pin_*", else device memory
+        (allocated in `stream`'s pool).  A buffer is replaced only by a larger one (sizes are powers of two), after the
+        device has finished with the old one."""
+        bufs = self.__dict__.setdefault("_stream_buffers", {})
+        buf = bufs.get((kind, slot))
+        if buf is None or buf.numel() < nbytes:
+            torch.cuda.synchronize(self.device)
+            size = 1 << max(20, (int(nbytes) - 1).bit_length())
+            if kind.startswith("pin_"):
+                buf = torch.empty(size, dtype=torch.uint8, pin_memory=True)
+            else:
+                # see rois_batches: a buffer another stream writes must not be a block the compute stream's tensors
+                # have just released, so it comes from that stream's pool
+                with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream()):
+                    buf = torch.empty(size, dtype=torch.uint8, device=self.device)
+                torch.cuda.synchronize(self.device)
+            bufs[(kind, slot)] = buf
+        return buf
+
+    def _stream(self, images, split, what, resize, max_batch, return_resized, scale, max_scale, window, compact_rows, after=None):
+        """The generator behind stream_rois_images / stream_images / stream_lines_images: run_stream over the batches of
+        stream_windows with these stages, on two slots used alternately --
+          pack     (worker thread) the batch's rows, row maps, sizes and im_info into the slot's pinned buffer
+                   (stream_layout), once the upload that last read that buffer has finished;
+          upload   one H2D of that buffer on the copy stream, once the compute that last read the slot's device buffer has
+                   finished;
+          compute  on the current stream: the front-end kernels, detect_packed and after(packed, items), as _images_batches
+                   runs them, into the slot's uint8 canvas; then on the result stream one D2H of the result (and, with
+                   return_resized, one of the uint8 canvas);
+          finish   waits for that D2H and splits it: split(host buffer, batch) -> one tuple per image.
+        The host blocks only in finish, for the batch it is about to yield."""
+        if not 1 <= int(max_batch) <= 64:
+            raise ValueError("%s: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)" % what)
+        window = 2 * int(max_batch) if window is None else int(window)
+        if window < 1:
+            raise ValueError("%s: window must be at least 1" % what)
+        if getattr(self, "_copy_stream", None) is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+            self._result_stream = torch.cuda.Stream(device=self.device)
+        copy_stream, result_stream = self._copy_stream, self._result_stream
+        main = torch.cuda.current_stream()
+        lut = self._mean_lut()
+        copied, computed, returned = [None, None], [None, None], [None, None]     # per slot: events of its last H2D / compute / D2H
+
+        def prepare(im, index):
+            a = im.numpy() if torch.is_tensor(im) else np.asarray(im)
+            return a, frontend_plan([a], resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg, first=index)[0]
+
+        def pack_on_host(batch, slot):          # calling thread: sizes only, and the pinned buffer (grow-only)
+            lay = stream_layout(batch.items, [im.shape[:2] for im in batch.images], compact_rows)
+            return lay, self._stream_buffer("pin_src", slot, lay.total), copied[slot]
+
+        def pack(batch, slot, staged):          # worker thread: row copies (numpy releases the GIL for them)
+            lay, pinned, free = staged
+            if free is not None:
+                free.synchronize()
+            stream_pack(pinned.numpy(), lay, batch)
+            return lay, pinned
+
+        def upload(batch, slot, packed):
+            lay, pinned = packed
+            dev = self._stream_buffer("src", slot, lay.total, copy_stream)
+            with torch.cuda.stream(copy_stream):
+                if computed[slot] is not None:
+                    copy_stream.wait_event(computed[slot])
+                dev[:lay.total].copy_(pinned[:lay.total], non_blocking=True)          # the batch's one H2D
+                copied[slot] = torch.cuda.Event()
+                copied[slot].record(copy_stream)
+            return lay, dev, copied[slot]
+
+        def compute(batch, slot, uploaded):
+            lay, dev, arrived = uploaded
+            items, (H, W) = batch.items, batch.canvas
+            B = len(items)
+            stream = N.stream_ptr()
+            main.wait_event(arrived)
+            if returned[slot] is not None:
+                main.wait_event(returned[slot])        # the D2H out of this slot's uint8 canvas
+            is_u8 = items[0].dtype == "|u1"
+            Hr, Wr = (H, W) if is_u8 else (max(p.resized[0] for p in items), max(p.resized[1] for p in items))
+            u8 = self._stream_buffer("u8", slot, B * Hr * Wr * 3)[:B * Hr * Wr * 3].view(B, Hr, Wr, 3)
+            hwp = np.array([im.shape[:2] + (im.shape[1],) for im in batch.images], np.int32)
+            fxy = np.array([[p.f, p.f] for p in items], np.float64)
+            resized_hw = np.array([p.resized for p in items], np.int32)
+            if lay.maps is None:
+                N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(dev), lay.map_base, N.ptr(lay.offsets), N.ptr(hwp), N.ptr(fxy),
+                                                           N.ptr(resized_hw), B, 3, N.ptr(u8), Hr, Wr, stream),
+                        "ctpn_resize_linear_u8_ragged")
+            else:
+                maps = dev[lay.map_base:lay.sizes_at].view(torch.int32)
+                N.check(N.lib.ctpn_resize_linear_u8_ragged_rows(N.ptr(dev), lay.map_base, N.ptr(lay.offsets), N.ptr(hwp),
+                                                                N.ptr(lay.stored), N.ptr(maps), maps.numel(), N.ptr(lay.maps),
+                                                                N.ptr(fxy), N.ptr(resized_hw), B, 3, N.ptr(u8), Hr, Wr, stream),
+                        "ctpn_resize_linear_u8_ragged_rows")
+            canvas = u8
+            if not is_u8:
+                canvas = self._workspace("stream_blob", B * H * W * 12)[:B * H * W * 12].view(torch.float32).view(B, H, W, 3)
+                boffs = np.arange(B, dtype=np.int64) * (Hr * Wr * 3)
+                bhwp = np.concatenate([resized_hw, np.full((B, 1), Wr, np.int32)], axis=1)
+                bfxy = np.array([[p.im_scale, p.im_scale] for p in items], np.float64)
+                blob_hw = np.array([p.blob for p in items], np.int32)
+                N.check(N.lib.ctpn_image_blob_f32_ragged(N.ptr(u8), B * Hr * Wr * 3, N.ptr(boffs), N.ptr(bhwp), N.ptr(bfxy),
+                                                         N.ptr(blob_hw), N.ptr(lut), B, N.ptr(canvas), H, W, stream),
+                        "ctpn_image_blob_f32_ragged")
+            tail = dev[lay.sizes_at:lay.total]
+            ints = tail[:16 * B].view(torch.int32)
+            packed = self.detect_packed(canvas, tail[16 * B:].view(torch.float32).view(B, 3), sizes=np.array([p.blob for p in items]),
+                                        device_sizes=(ints[:2 * B].view(B, 2), ints[2 * B:].view(B, 2)))
+            result = packed if after is None else after(packed, items)
+            computed[slot] = torch.cuda.Event()
+            computed[slot].record(main)
+            nbytes = result.numel() * result.element_size()
+            with torch.cuda.stream(result_stream):
+                result_stream.wait_event(computed[slot])
+                out_h = self._stream_buffer("pin_out", slot, nbytes)[:nbytes].view(result.dtype)
+                out_h.copy_(result, non_blocking=True)                                  # one D2H: the packed results
+                res_h = None
+                if return_resized:                                                      # and one for the resize_im outputs
+                    res_h = self._stream_buffer("pin_u8", slot, u8.numel())[:u8.numel()].view(B, Hr, Wr, 3)
+                    res_h.copy_(u8, non_blocking=True)
+                returned[slot] = torch.cuda.Event()
+                returned[slot].record(result_stream)
+            return out_h, res_h, returned[slot], (packed, result)       # the device results live until the D2H has run
+
+        def finish(batch, handle):
+            out_h, res_h, ev, _keep = handle
+            ev.synchronize()
+            per_image = split(out_h, batch)
+            if res_h is not None:
+                rn = res_h.numpy()
+                per_image = [t + (rn[k, :p.resized[0], :p.resized[1]].copy(),) for k, (t, p) in enumerate(zip(per_image, batch.items))]
+            return per_image
+
+        def drain():
+            for st in (copy_stream, main, result_stream):
+                st.synchronize()
+            self._streaming = False
+
+        def stream():
+            if getattr(self, "_streaming", False):
+                raise RuntimeError("%s: another stream of this engine is still open (its slots are in use); close it first" % what)
+            self._streaming = True
+            yield from run_stream(stream_windows(images, window, max_batch, prepare), pack_on_host, pack, upload, compute, finish,
+                                  drain)
+
+        return stream()
+
+    def stream_rois_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, window=None,
+                           compact_rows=True):
+        """rois_images for any iterable of raw HxWx3 uint8 BGR images (e.g. a generator that decodes files), as a generator:
+        yields, in input order, the tuple rois_images returns for each image -- bit-identical to it -- while later images
+        are still being pulled, packed, uploaded and computed (see _stream for the stages that overlap).  window: how
+        many images are pulled from the iterable before their ragged batches are planned (default 2 * max_batch); it
+        bounds the memory held and, like max_batch, changes which images share a batch, never a result.  A camera-size
+        photo is uploaded as the rows resize_im reads only (FrontendStep.rows; compact_rows=False uploads every image
+        whole).  A bad image raises frontend_plan's ValueError when the stream reaches it, after the results of all images
+        before it.  Closing the generator early waits for the work in flight and leaves the engine ready for any other
+        call; one stream per engine can be open at a time."""
+        rows = self.result_rows()
+
+        def split(out_h, batch):
+            return [(r, p.im_scale, p.f) for r, p in zip(self._split_results(out_h, len(batch.items), rows), batch.items)]
+
+        return self._stream(images, split, "stream_rois_images", resize, max_batch, return_resized, scale, max_scale, window,
+                            compact_rows)
+
+    def stream_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, window=None,
+                      compact_rows=True):
+        """detect_images as a generator over any iterable of raw photos: see stream_rois_images."""
+        rows = self.result_rows()
+
+        def split(out_h, batch):
+            return [(r[:, 0], r[:, 1:5] / np.float64(p.im_scale), p.f)
+                    for r, p in zip(self._split_results(out_h, len(batch.items), rows), batch.items)]
+
+        return self._stream(images, split, "stream_images", resize, max_batch, return_resized, scale, max_scale, window,
+                            compact_rows)
+
+    def stream_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
+                            cfg=None, window=None, compact_rows=True):
+        """detect_lines_images as a generator over any iterable of raw photos: see stream_rois_images; the connector runs
+        on each batch's rois on the device and only the lines come back.  Raises CtpnError where detect_lines_images does."""
+        if mode not in ("H", "O"):
+            raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
+        rows = self.result_rows()
+
+        def split(out_h, batch):
+            hw = [p.resized for p in batch.items]
+            lines = self.split_lines(*self.unpack_lines(out_h.numpy(), len(hw), rows), im_hw=hw)
+            return [(ln, p.f) for ln, p in zip(lines, batch.items)]
+
+        return self._stream(images, split, "stream_lines_images", resize, max_batch, return_resized, scale, max_scale, window,
+                            compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg))
+
+    def _connect(self, packed, items, mode, cfg):
+        """The text-line connector on one batch's packed rois -> the packed lines (unpack_lines), on the device."""
+        B, rows = len(items), self.result_rows()
+        rois, count = self.unpack(packed, B, rows)
+        res = torch.empty(B * rows * 9 + B, dtype=torch.float64, device=self.device)
+        self.text_lines(rois, count, [p.resized for p in items], [p.im_scale for p in items], mode, cfg,
+                        out=self.unpack_lines(res, B, rows))
+        return res
 
     def detect(self, image, im_scale=1.0):
         """Single image [H,W,3] -> (scores, boxes); the test_ctpn() contract."""
@@ -826,14 +1040,26 @@ def ragged_plan(shapes, dtypes, max_batch=32):
     return plan
 
 
-FrontendStep = collections.namedtuple("FrontendStep", "f resized im_scale blob dtype")
+FrontendStep = collections.namedtuple("FrontendStep", "f resized im_scale blob dtype rows", defaults=(None,))
+
+
+def frontend_rows(h, f_y, out_h):
+    """The source rows that resize_im's cv2.resize of an h-row uint8 image by f_y to out_h rows reads: sorted, unique,
+    int64.  INTER_LINEAR takes output row d from rows s and s + 1, s = floor(float32((d + 0.5) * (1 / f_y) - 0.5)), both
+    clamped to [0, h - 1]; an exact 1/2 is routed to INTER_AREA, which reads every row."""
+    h, out_h = int(h), int(out_h)
+    scale = 1.0 / float(f_y)
+    if scale == 2.0:
+        return np.arange(h, dtype=np.int64)
+    s = np.floor(((np.arange(out_h, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)).astype(np.int64)
+    return np.unique(np.clip(np.concatenate([s, s + 1]), 0, h - 1))
 
 
 def _cv_round_size(h, w, s):
     return int(np.rint(float(h) * s)), int(np.rint(float(w) * s))        # cvRound: round half to even, in float64
 
 
-def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None):
+def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None, first=0):
     """What the demo's host front-end does to each image, computed on the host: shapes is a list of HxWx3 uint8 images
     (anything with .shape and .dtype) or of (H, W[, 3]) tuples.  Per image a FrontendStep of
       f         the resize_im factor (ctpn/demo.py: short side -> scale unless the long side would exceed max_scale;
@@ -842,14 +1068,16 @@ def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None):
       im_scale  _get_image_blob's scale (lib/fast_rcnn/test.py _im_scale: SCALES[0] / short side, or MAX_SIZE / long side
                 when np.round(im_scale * long side) > MAX_SIZE; cfg: SCALES and MAX_SIZE, default DEFAULT_CFG),
       blob      the (h, w) of the blob the network sees,
-      dtype     '|u1' when im_scale == 1 (the uint8 image is the blob), else '<f4' (the float32 rescale).
-    Raises ValueError when an image is not HxWx3 uint8, a resize would be empty or a blob side would be under 16."""
+      dtype     '|u1' when im_scale == 1 (the uint8 image is the blob), else '<f4' (the float32 rescale),
+      rows      the source rows resize_im reads (frontend_rows, as a tuple) when they are at most 3/4 of the image -- a
+                streamed upload then sends only those (Engine.stream_rois_images) -- or None: send the image densely.
+    Error messages number the images from `first` (a stream plans its images one at a time).  Raises ValueError when an image is not HxWx3 uint8, a resize would be empty or a blob side would be under 16."""
     c = dict(DEFAULT_CFG)
     if cfg:
         c.update(cfg)
     target, max_size = float(c["SCALES"][0]), float(c["MAX_SIZE"])
     out = []
-    for i, s in enumerate(shapes):
+    for i, s in enumerate(shapes, int(first)):
         if hasattr(s, "shape") and hasattr(s, "dtype"):
             if len(s.shape) != 3 or s.shape[2] != 3 or str(s.dtype) not in ("uint8", "torch.uint8"):
                 raise ValueError("frontend_plan: image %d must be HxWx3 uint8 (got %s %s)" % (i, tuple(s.shape), s.dtype))
@@ -874,8 +1102,151 @@ def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None):
         bh, bw = (rh, rw) if im_scale == 1.0 else _cv_round_size(rh, rw, im_scale)
         if bh < 16 or bw < 16:
             raise ValueError("frontend_plan: image %d (%dx%d) gives a %dx%d blob; both sides must be at least 16" % (i, h, w, bh, bw))
-        out.append(FrontendStep(f, (rh, rw), im_scale, (bh, bw), "|u1" if im_scale == 1.0 else "<f4"))
+        rows = None
+        if f < 0.5:            # at 1/2 and above the two taps of consecutive output rows cover every source row
+            live = frontend_rows(h, f, rh)
+            if 4 * len(live) <= 3 * h:
+                rows = tuple(int(r) for r in live)
+        out.append(FrontendStep(f, (rh, rw), im_scale, (bh, bw), "|u1" if im_scale == 1.0 else "<f4", rows))
     return out
+
+
+# ---- streamed photos: the parts of Engine._stream that need no device ---------------------------------------------------
+StreamBatch = collections.namedtuple("StreamBatch", "idxs items images canvas")
+# One batch's upload: [the images' rows, back to back][row maps, int32][blob sizes, int32 B x 2][feature sizes, int32 B x 2]
+# [im_info, float32 B x 3].  offsets / stored: per image, where its rows start (bytes) and how many it sends; rows: which
+# (None: all); map_base: where the sources end and the maps start (a multiple of 4); maps: per image, where its map starts
+# (int32 elements from map_base), or None when no image of the batch is compacted and there are no maps; sizes_at, total.
+StreamLayout = collections.namedtuple("StreamLayout", "offsets stored rows map_base maps sizes_at total")
+
+
+def stream_layout(items, shapes, compact_rows=True):
+    """Where everything of one batch goes in its upload buffer: items are the batch's FrontendSteps, shapes its images'
+    (h, w).  An image is sent as its FrontendStep.rows when it has them (and compact_rows), else whole; if any image of the
+    batch is compacted, every image gets a row map (the identity for a whole one)."""
+    rows = [p.rows if compact_rows else None for p in items]
+    stored = np.array([h if r is None else len(r) for (h, w), r in zip(shapes, rows)], np.int32)
+    nbytes = [int(n) * int(w) * 3 for n, (h, w) in zip(stored, shapes)]
+    offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
+    map_base = (int(sum(nbytes)) + 3) & ~3
+    maps, sizes_at = None, map_base
+    if any(r is not None for r in rows):
+        heights = [int(h) for h, w in shapes]
+        maps = np.cumsum([0] + heights[:-1]).astype(np.int64)
+        sizes_at += 4 * sum(heights)
+    return StreamLayout(offsets, stored, rows, map_base, maps, sizes_at, sizes_at + 28 * len(items))
+
+
+def stream_pack(buf, lay, batch):
+    """Fills a batch's upload buffer (uint8 ndarray of at least lay.total bytes) as stream_layout laid it out."""
+    B = len(batch.items)
+    for k, im in enumerate(batch.images):
+        h, w = im.shape[:2]
+        n, r = int(lay.stored[k]), lay.rows[k]
+        dst = buf[lay.offsets[k]:lay.offsets[k] + n * w * 3].reshape(n, w, 3)
+        if r is None:
+            dst[...] = im
+        else:
+            np.take(im, r, axis=0, out=dst, mode="clip")
+        if lay.maps is not None:          # original row -> stored row; rows that are not stored are never looked up
+            m = buf[lay.map_base + 4 * lay.maps[k]:lay.map_base + 4 * (lay.maps[k] + h)].view(np.int32)
+            if r is None:
+                m[:] = np.arange(h, dtype=np.int32)
+            else:
+                m[:] = 0
+                m[np.asarray(r)] = np.arange(n, dtype=np.int32)
+    blobs = np.array([p.blob for p in batch.items], np.int32)
+    tail = buf[lay.sizes_at:lay.total]
+    tail[:8 * B].view(np.int32)[:] = blobs.ravel()
+    tail[8 * B:16 * B].view(np.int32)[:] = (blobs >> 4).ravel()
+    tail[16 * B:].view(np.float32)[:] = np.array([[p.blob[0], p.blob[1], p.im_scale] for p in batch.items], np.float32).ravel()
+
+
+def stream_windows(images, window, max_batch, prepare):
+    """The ragged batches of a stream of images: pulls up to `window` images from the iterable, prepare(image, index) ->
+    (array, FrontendStep) for each, plans them (ragged_plan) and yields their StreamBatches (idxs: positions in the stream);
+    then the next window.  A ValueError of prepare is raised after the batches of the images before that image."""
+    it = iter(images)
+    first = 0
+    while True:
+        arrays, steps, bad = [], [], None
+        for im in it:
+            try:
+                a, p = prepare(im, first + len(arrays))
+            except ValueError as e:
+                bad = e
+                break
+            arrays.append(a)
+            steps.append(p)
+            if len(arrays) == window:
+                break
+        for idxs, canvas in ragged_plan([p.blob for p in steps], [p.dtype for p in steps], max_batch):
+            yield StreamBatch([first + i for i in idxs], [steps[i] for i in idxs], [arrays[i] for i in idxs], canvas)
+        if bad is not None:
+            raise bad
+        if len(arrays) < window:
+            return
+        first += len(arrays)
+
+
+def run_stream(batches, stage, pack, upload, compute, finish, drain):
+    """Drives a stream of StreamBatches through a two-slot pipeline and yields every image's result in stream order.
+    Batch k uses slot k & 1.  stage(batch, slot) runs on the calling thread and pack(batch, slot, staged) on a worker
+    thread, two batches ahead of the compute; upload(batch, slot, packed) one batch ahead; compute(batch, slot, uploaded)
+    enqueues batch k and returns a handle; finish(batch, handle) -> one result per image, called one batch behind, is the
+    only stage that may wait for the device.  An exception of `batches` is raised after every batch before it has been
+    yielded.  However the generator ends (exhausted, closed or raising), the worker thread is joined and drain() is
+    called."""
+    import concurrent.futures
+    pool = concurrent.futures.ThreadPoolExecutor(max_workers=1, thread_name_prefix="ctpn-stream-pack")
+    packing, uploaded = collections.deque(), collections.deque()
+    state = {"k": 0, "error": None, "more": True}
+
+    def pull():
+        if not state["more"]:
+            return
+        try:
+            batch = next(batches)
+        except StopIteration:
+            state["more"] = False
+            return
+        except Exception as e:
+            state["more"], state["error"] = False, e
+            return
+        slot = state["k"] & 1
+        state["k"] += 1
+        packing.append((batch, slot, pool.submit(pack, batch, slot, stage(batch, slot))))
+
+    def upload_next():
+        if packing:
+            batch, slot, fut = packing.popleft()
+            uploaded.append((batch, slot, upload(batch, slot, fut.result())))
+
+    ready, next_out, pending = {}, 0, None
+    try:
+        pull()
+        upload_next()
+        pull()
+        while uploaded or pending is not None:
+            this = None
+            if uploaded:
+                batch, slot, up = uploaded.popleft()
+                this = (batch, compute(batch, slot, up))
+                upload_next()
+                pull()
+            if pending is not None:
+                for i, r in zip(pending[0].idxs, finish(*pending)):
+                    ready[i] = r
+                while next_out in ready:
+                    yield ready.pop(next_out)
+                    next_out += 1
+            pending = this
+        if state["error"] is not None:
+            raise state["error"]
+    finally:
+        pool.shutdown(wait=True, cancel_futures=True)
+        batches.close()
+        drain()
 
 
 # the 38 variables of the VGGnet_test graph (SURVEY.md App. A.2); a TF checkpoint also holds optimizer slots etc.
