@@ -41,7 +41,9 @@ class Engine:
     def __init__(self, weights=None, planes=2, device=0, cfg=None, conv_simt=False, keep_activations=False, streams=1, mode=None,
                  graph_max_batch=4):
         """graph_max_batch: batches of up to this many images run as a replayed CUDA graph per (shape, dtype) bucket (the ~25
-        kernel launches of a step cost more than the kernels themselves at batch 1); 0 disables graphs."""
+        kernel launches of a step cost more than the kernels themselves at batch 1); 0 disables graphs.
+        streams: run each batch as this many sub-batches on side streams (detect_packed), with results bit-identical to
+        streams=1; a forward that calibrates the F16F8 scales runs unsplit, so that they come from the whole batch."""
         if mode is not None:
             planes = self.MODES[mode]
         self.graph_max_batch = int(graph_max_batch)
@@ -66,6 +68,7 @@ class Engine:
         self._pinned = {}
         self.streams = int(streams)
         self._side = []
+        self._calibrated = False      # mirrors the library's F16F8 calibration state (see detect_packed)
         if weights is not None:
             self.load_weights(weights)
 
@@ -84,6 +87,7 @@ class Engine:
         if isinstance(weights, str):
             weights = load_weight_file(weights)
         self._graphs.clear()          # captured graphs hold the old weight buffers' addresses
+        self._calibrated = False      # new weights re-arm the F16F8 calibration
         for name, arr in weights.items():
             a = np.ascontiguousarray(arr, dtype=np.float32)
             N.check(N.lib.ctpn_net_set_weight(self._net, name.encode(), N.ptr(a), a.size), "ctpn_net_set_weight(%s)" % name)
@@ -151,6 +155,7 @@ class Engine:
             sz = self._sizes_device(sizes, B, H, W, device=sizes_device)
             N.check(N.lib.ctpn_net_forward_ragged(self._net, N.ptr(images), int(is_f32), N.ptr(sz), B, H, W, N.ptr(cls),
                                                   N.ptr(bbox), N.ptr(ws), ws.numel(), N.stream_ptr()), "ctpn_net_forward_ragged")
+        self._calibrated = True
         return cls, bbox
 
     def recalibrate(self):
@@ -161,6 +166,7 @@ class Engine:
         past which the element saturates in fp16 too and its error is unbounded.  So calibrate on representative images --
         not on a flat warm-up image -- and call this again when the input distribution changes."""
         N.check(N.lib.ctpn_net_set_option(self._net, b"recalibrate", 1), "set_option")
+        self._calibrated = False
         self._graphs.clear()          # captured graphs hold the old scales as kernel arguments
 
     def tap(self, name):
@@ -241,7 +247,8 @@ class Engine:
         rows = self.result_rows()
         packed = torch.empty(B * rows * 5 + B, dtype=torch.float32, device=self.device)
         rois, count = self.unpack(packed, B, rows)
-        n = min(self.streams, B)
+        # a forward that calibrates the F16F8 scales runs unsplit: the scales must come from the whole batch, as with streams=1
+        n = min(self.streams, B) if self._calibrated or self.planes != self.MODES["f16f8"] else 1
         if n <= 1:
             cls, bbox = self.forward_heads(images, ws_key="net" + ws_tag, sizes=sizes, sizes_device=sz_d)
             self.proposals(cls, bbox, im_info, cls_is_logit=True, ws_key="prop" + ws_tag, out=(rois, count),
@@ -455,17 +462,28 @@ class Engine:
         if pending is not None:
             yield finish(pending)
 
-    def detect_lines_batches(self, batches, mode="H", im_info=None, workers=8, gather=False, cfg=None):
+    def detect_lines_batches(self, batches, mode="H", im_info=None, workers=8, gather=False, cfg=None, im_hw=None):
         """The whole ctpn() call chain (demo.py:55-68 minus file I/O) for a stream of host batches: rois_batches() on the
         GPU, then TextDetector.detect of every image in the library's host connector (ctpn_text_lines_host, which
         releases the GIL) on a pool of `workers` threads, one batch behind the GPU.  With gather=True (multi-GPU) the rois of
         all ranks are gathered as in rois_batches and every rank runs the connector on its own shard.  Yields, per batch, a list of
-        float64 [m,9] text-line arrays (x1,y1,x2,y2,x3,y3,x4,y4,score) in the frame of the blob divided by im_scale."""
+        float64 [m,9] text-line arrays (x1,y1,x2,y2,x3,y3,x4,y4,score) in the frame im_hw = (h, w) of the image the blobs were
+        made from (resize_im's output): text_lines(rois[:, 1:5] / np.float64(scale), rois[:, 0], im_hw, mode, cfg), as
+        test_ctpn and TextDetector compute them, with the scale im_info[0, 2] as given (pass im_info as float64 to keep an
+        inexact scale such as 1000 / 1100 exactly as test_ctpn has it).  im_hw=None: the frame is each batch's (H, W), which
+        needs scale 1 -- the blob's size divided by the scale does not give the image's size back in general."""
         from concurrent.futures import ThreadPoolExecutor
         from .textlines import text_lines
 
-        def lines_of(rois, size, scale):
-            return text_lines(rois[:, 1:5] / np.float32(scale), rois[:, 0], size, mode, cfg)
+        scale = 1.0 if im_info is None else float(np.asarray(im_info).reshape(-1, 3)[0, 2])
+        if im_hw is None and scale != 1.0:
+            raise ValueError("detect_lines_batches: im_hw= (the frame of the lines) is needed when the scale is not 1 (got %r)" % scale)
+        frame = None if im_hw is None else tuple(int(v) for v in im_hw)
+        if frame is not None and len(frame) != 2:
+            raise ValueError("detect_lines_batches: im_hw must be one (h, w) pair (got %r)" % (im_hw,))
+
+        def lines_of(rois, size):
+            return text_lines(rois[:, 1:5] / np.float64(scale), rois[:, 0], size, mode, cfg)
 
         batches = iter(batches)
         shapes = []
@@ -487,9 +505,8 @@ class Engine:
             if shard is not None:      # every rank holds all ranks' rois after the gather; each builds the lines of its own shard
                 per = len(rois_list) // shard[1]
                 rois_list = rois_list[shard[0] * per:(shard[0] + 1) * per]
-            H, W = shapes[k]
-            scale = 1.0 if im_info is None else float(np.asarray(im_info, np.float32).reshape(-1, 3)[0, 2])
-            futs = [pool.submit(lines_of, r, (int(round(H / scale)), int(round(W / scale))), scale) for r in rois_list]
+            size = shapes[k] if frame is None else frame
+            futs = [pool.submit(lines_of, r, size) for r in rois_list]
             if pending is not None:
                 yield [f.result() for f in pending]
             pending = futs
