@@ -16,15 +16,17 @@
 //     wgmma, or k32 for e4m3) and keep one group of MMAs in flight; a stage is released when its group completes.
 //     With P > 1 planes the plane-0 x plane-0 products go to a "main" accumulator and all cross-plane
 //     products to a second one (the tensor core truncates when adding into float32; see DESIGN.md).
-//   * epilogue (both consumer warpgroups; thread = pixel, a set of 4 warps takes every other 32-column chunk): the
-//     accumulator fragments go through a float32 staging buffer -> +bias -> ReLU -> optional fused 2x2 max-pool (warp
-//     shuffles: the window of a pixel lives in lanes l, l^1, l^8, l^9) -> re-split into planes (cvt.rn.bf16x2.f32) ->
-//     transpose through swizzled shared memory -> 16-byte stores that cover one pixel's 64 contiguous bytes with 4 lanes
-//     (or float32 output).
+//   * epilogue (thread = pixel): the combined accumulators go through a float32 staging buffer, 64 channels at a time ->
+//     +bias -> ReLU -> optional fused 2x2 max-pool (warp shuffles: the window of a pixel lives in lanes l, l^1, l^8, l^9)
+//     -> re-split into planes (cvt.rn.bf16x2.f32) -> transpose through swizzled shared memory -> 16-byte stores that
+//     cover one pixel's 64 contiguous bytes with 4 lanes (or float32 output).
 // Small and promoted 3x3 layers run as 2-CTA clusters that share every weight tile by TMA multicast (template parameter MC;
 // CTPN_TC_MCAST=0 selects the single-CTA variant everywhere); large unpromoted ones run one CTA per SM (conv_tc_run).
-// Persistent CTAs (one per SM), warp-specialised: warp 0 weight (B) producer, warp 1 activation (A) producer,
-// warpgroups 1 and 2 MMAs + epilogue.  Reference: lib/networks/network.py:160-196.
+// Persistent CTAs (one per SM), warp-specialised: warp 0 weight (B) producer, warp 1 activation (A) producer, warpgroups
+// 1 and 2 MMAs, warpgroup 3 the epilogue: the MMA warpgroups hand each finished tile over through the staging buffer in
+// 64-channel halves (an mbarrier full / empty pair) and start the next tile's MMAs while warpgroup 3 converts and stores
+// it.  The promoted kernels (PR = 1: three accumulator arrays, no registers left for a fourth warpgroup) run the same
+// epilogue on the two MMA warpgroups after each tile.  Reference: lib/networks/network.py:160-196.
 #include <cuda.h>
 
 #include <algorithm>
@@ -75,16 +77,192 @@ struct ConvTcParams {
   const int *ext;
   int ext_shift, ext_n;
   double work;              // algorithmic FLOPs of the call (profiling label only)
-  int stage_small;          // 1: 512-byte store-transpose block per epilogue warp (8 pixels per round)
   int promote_every;        // test library only (CTPN_TC_PROMOTE): pipeline steps per promoted main chain (product: 1)
 };
 
-constexpr int kTcThreads = 384;   // warpgroup 0: producers (warp 0 weights, warp 1 activations); 1 and 2: MMAs + epilogue
+// warpgroup 0: producers (warp 0 weights, warp 1 activations); 1 and 2: MMAs; 3: epilogue.  PR = 1: 1 and 2 run MMAs and
+// the epilogue.
+// EW: the schedule with a dedicated epilogue warpgroup.  Not for the promoted kernels, and not at BN = 256: ptxas compiles a
+// 512-thread kernel's m64n256 wgmma (128 accumulator registers + operands) against the launch's 128 registers per thread,
+// whatever setmaxnreg grants the MMA warpgroups.
+template <int BN, int PR> constexpr bool kEpiWarpgroup = !PR && BN <= 128;
+template <int BN, int PR> constexpr int kTcThreads = kEpiWarpgroup<BN, PR> ? 512 : 384;
 constexpr int kMaxStages = 8;
-constexpr int kCtrlBytes = 8 * (4 * kMaxStages) + 16;
-constexpr int kStagePitch = 64;                    // bytes per pixel row of the epilogue store staging; 16-B chunks are
-                                                   // XOR-swizzled by (row >> 1) & 3: conflict-free writes AND reads
+constexpr int kCtrlBytes = 8 * (4 * kMaxStages) + 16;   // the four stage rings' barriers + the epilogue handoff pair
 constexpr int kEpiBytes = 2 * 128 * 32 * 4;        // float32 staging of two 32-channel chunks of the 128-pixel tile
+constexpr int kXposeBytes = 4 * 512;               // epilogue warpgroup: a 512-byte store-transpose block per warp
+
+// Where the epilogue thread of tile pixel m (lane = m & 31) writes, for pixel tile mt.  Warp-collective (ballot, shuffles).
+struct EpiPixel {
+  bool ok, live;        // ok: inside the output; live = false: stored as zero (a stacked pad row, or outside a ragged extent)
+  int oy, ox;
+  long long pix;        // output pixel index
+  unsigned okmask;      // the warp's ok lanes
+  long long spix[4];    // pixel of lane it * 8 + (lane >> 2): the transposed stores
+};
+
+__device__ __forceinline__ void epi_pixel(const ConvTcParams &p, int mt, int m, int lane, EpiPixel &e) {
+  const int th = m >> p.tw_log2, tw = m & (p.TW - 1);
+  const int tiles_per_img = p.tiles_x * p.tiles_y;
+  const int b = mt / tiles_per_img, r = mt % tiles_per_img;
+  const int y = (r / p.tiles_x) * p.TH + th, x = (r % p.tiles_x) * p.TW + tw;
+  e.live = true;
+  int ob = b;
+  if (p.flags & CTPN_F_POOL) {
+    e.oy = y >> 1; e.ox = x >> 1;
+    e.ok = !(th & 1) && !(tw & 1) && e.oy < p.Ho && e.ox < p.Wo;
+  } else {
+    e.oy = y; e.ox = x;
+    e.ok = y < p.H && x < p.W;
+    if (p.in_stack_h) {       // stacked input: y runs over the whole stack (the kernel sees one image of B * in_stack_h rows)
+      ob = y / p.in_stack_h;
+      e.oy = y - ob * p.in_stack_h;
+      e.live = e.oy < p.in_stack_h - 1;
+      if (!p.out_stacked) e.ok = e.ok && e.live;
+    }
+  }
+  if (p.ext) {     // ragged batch: zero outside the image's extent at the output level (with a pool: the whole window)
+    const int ib = min(ob, p.ext_n - 1);
+    e.live = e.live && e.oy < (__ldg(p.ext + 2 * ib) >> p.ext_shift) && e.ox < (__ldg(p.ext + 2 * ib + 1) >> p.ext_shift);
+  }
+  e.pix = ((long long)ob * p.out_rows + e.oy) * p.Wo + e.ox;
+  // coalesced plane stores: the warp's 32-pixel x 32-channel block is transposed through shared memory so
+  // that 4 consecutive lanes write the 64 contiguous bytes of one pixel (full 32-B sectors) instead of every
+  // lane writing 16 B of its own pixel.  Lane l stores for pixels (l >> 2) + 8 * it, 16-byte chunk l & 3.
+  e.okmask = __ballot_sync(0xffffffffu, e.ok);
+#pragma unroll
+  for (int it = 0; it < 4; ++it) {
+    const long long hi = __shfl_sync(0xffffffffu, (int)(e.pix >> 32), it * 8 + (lane >> 2));
+    const unsigned lo = __shfl_sync(0xffffffffu, (unsigned)(e.pix & 0xffffffffll), it * 8 + (lane >> 2));
+    e.spix[it] = (hi << 32) | lo;
+  }
+}
+
+// Each lane holds 64 bytes (w) of its own pixel; lane l stores 16-byte piece l & 3 of pixels (l >> 2) + 8 * it at
+// obase + spix[it] * row_bytes.  small = 0: one 2-KB transpose block (the warp's 32 pixels at once); 1: a 512-byte block,
+// 8 pixels per round.  16-byte pieces are XOR-swizzled by (row >> 1) & 3: conflict-free writes and reads.
+__device__ __forceinline__ void store_transposed(uint4 *stage_w, const uint32_t (&w)[16], uint8_t *obase, long long row_bytes,
+                                                 const EpiPixel &e, bool st_ok, bool small, int lane) {
+  const int j = lane & 3;
+  if (!small) {
+    __syncwarp();     // previous readers of the staging block are done
+#pragma unroll
+    for (int q = 0; q < 4; ++q) stage_w[lane * 4 + (q ^ ((lane >> 1) & 3))] = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+    __syncwarp();
+    if (st_ok) {
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {
+        const int pp = it * 8 + (lane >> 2);
+        const uint4 val = stage_w[pp * 4 + (j ^ ((pp >> 1) & 3))];
+        if ((e.okmask >> pp) & 1u) *reinterpret_cast<uint4 *>(obase + e.spix[it] * row_bytes) = val;
+      }
+    }
+  } else {
+    // lanes 8 it .. 8 it + 7 deposit their 64 bytes, all 32 lanes then store one 16-byte piece each
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      __syncwarp();
+      if ((lane >> 3) == it) {
+        const int row = lane & 7;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) stage_w[row * 4 + (q ^ ((row >> 1) & 3))] = make_uint4(w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+      }
+      __syncwarp();
+      const int row = lane >> 2, pp = it * 8 + row;
+      const uint4 val = stage_w[row * 4 + (j ^ ((row >> 1) & 3))];
+      if (st_ok && ((e.okmask >> pp) & 1u)) *reinterpret_cast<uint4 *>(obase + e.spix[it] * row_bytes) = val;
+    }
+  }
+}
+
+// The epilogue of one 32-channel chunk (output channels c0 .. c0 + 31) of one pixel: v = the combined accumulators.
+// +bias -> ReLU (unless the MMA warpgroups applied them: bias_relu = false) -> live mask -> optional fused 2x2 max-pool ->
+// F16F8 / bf16 planes / float32 stores.
+template <int P, int F8>
+__device__ __forceinline__ void epi_chunk(const ConvTcParams &p, const EpiPixel &e, float (&v)[32], int c0, uint4 *stage_w,
+                                          bool small, bool bias_relu, int lane) {
+  const bool pool = (p.flags & CTPN_F_POOL) != 0, relu = (p.flags & CTPN_F_RELU) != 0;
+  const bool out_f32 = (p.flags & CTPN_F_OUT_F32) != 0;
+  if (bias_relu) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const float4 bq = __ldg(reinterpret_cast<const float4 *>(p.bias + c0) + q);
+      v[4 * q + 0] += bq.x;
+      v[4 * q + 1] += bq.y;
+      v[4 * q + 2] += bq.z;
+      v[4 * q + 3] += bq.w;
+    }
+    if (relu) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
+    }
+  }
+  if (!e.live) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) v[i] = 0.f;
+  }
+  if (pool) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      v[i] = fmaxf(v[i], __shfl_xor_sync(0xffffffffu, v[i], 1));
+      v[i] = fmaxf(v[i], __shfl_xor_sync(0xffffffffu, v[i], p.TW));
+    }
+  }
+  if (F8 && pool && !out_f32 && !(p.flags & CTPN_F_OUT_BF16X2)) {
+    // Pooled F16F8 output without staging: after the shuffles all four lanes of a 2x2 window (l, l^1, l^8, l^9) hold the
+    // pooled value, so each takes one quarter (8 channels) of the chunk: a quarter of the conversions, and the four
+    // lanes' stores form 64 contiguous bytes of the fp16 plane and 32 + 32 of the e4m3 plane (full sectors).
+    const int j = (lane & 1) | ((lane >> 2) & 2);
+    float x[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) x[k] = j == 0 ? v[k] : j == 1 ? v[8 + k] : j == 2 ? v[16 + k] : v[24 + k];
+    const bool okw = e.oy < p.Ho && e.ox < p.Wo;     // (pix already points into the stacked frame when out_rows = Ho + 1)
+    uint4 hw;
+    uint2 qv, qr;
+    f16f8_quad(x[0], x[1], x[2], x[3], p.out_s, p.out_t, p.out_rs, hw.x, hw.y, qv.x, qr.x);
+    f16f8_quad(x[4], x[5], x[6], x[7], p.out_s, p.out_t, p.out_rs, hw.z, hw.w, qv.y, qr.y);
+    if (okw && c0 < p.Cout && !CTPN_DBG(p, 8)) {
+      uint8_t *o0 = reinterpret_cast<uint8_t *>(p.out) + e.pix * p.Cout * 2;
+      uint8_t *o1 = o0 + p.out_plane_stride * 2 + (long long)(c0 >> 6) * 128 + (c0 & 63) + j * 8;
+      *reinterpret_cast<uint4 *>(o0 + (long long)c0 * 2 + j * 16) = hw;
+      *reinterpret_cast<uint2 *>(o1) = qv;
+      *reinterpret_cast<uint2 *>(o1 + 64) = qr;
+    }
+  } else if (F8 && !out_f32 && !(p.flags & CTPN_F_OUT_BF16X2)) {
+    // F16F8 planes: fp16 words, then the e4m3 copies of the values and of the residuals (8 + 8 words)
+    uint32_t wh[16], wq[16];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      f16f8_quad(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3], p.out_s, p.out_t, p.out_rs, wh[2 * i], wh[2 * i + 1], wq[i], wq[8 + i]);
+    }
+    const int j = lane & 3;
+    const bool st_ok = c0 < p.Cout && !CTPN_DBG(p, 8);
+    // plane 0: 64 contiguous bytes per pixel (32 fp16).  plane 1: the pixel's 128-byte block of channel block
+    // c0 / 64 holds values at +0 and residuals at +64; this chunk owns 32 bytes of each
+    uint8_t *obase = reinterpret_cast<uint8_t *>(p.out);
+    store_transposed(stage_w, wh, obase + (long long)c0 * 2 + j * 16, (long long)p.Cout * 2, e, st_ok, small, lane);
+    store_transposed(stage_w, wq, obase + p.out_plane_stride * 2 + (long long)(c0 >> 6) * 128 + (c0 & 63) + (j >> 1) * 64 + (j & 1) * 16,
+                     (long long)p.Cout * 2, e, st_ok, small, lane);
+  } else if (!out_f32) {
+    uint32_t w[P][16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      uint32_t t[P];
+      split_planes2<P>(v[2 * i], v[2 * i + 1], t);
+#pragma unroll
+      for (int pl = 0; pl < P; ++pl) w[pl][i] = t[pl];
+    }
+#pragma unroll
+    for (int pl = 0; pl < P; ++pl) {
+      uint8_t *obase = reinterpret_cast<uint8_t *>(reinterpret_cast<__nv_bfloat16 *>(p.out) + (long long)pl * p.out_plane_stride + c0 + (lane & 3) * 8);
+      store_transposed(stage_w, w[pl], obase, (long long)p.Cout * 2, e, c0 < p.Cout && !CTPN_DBG(p, 8), small, lane);
+    }
+  } else if (e.ok && c0 < p.Cout && !CTPN_DBG(p, 8)) {
+    float4 *dst = reinterpret_cast<float4 *>(reinterpret_cast<float *>(p.out) + e.pix * p.Cout + c0);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+  }
+}
 
 // MC = 1: launched as 2-CTA clusters.  The two CTAs of a cluster work on two pixel tiles of the SAME output-channel tile in
 // lock step; each loads half of every weight (B) tile and TMA-multicasts it into both CTAs' shared memory, which halves the
@@ -97,12 +275,16 @@ constexpr int kEpiBytes = 2 * 128 * 32 * 4;        // float32 staging of two 32-
 // block, K = 64) and each step's partial sum is added into a third register array with round-to-nearest float32 adds, so
 // the tensor core's truncating adds run over chains of 4 MMAs instead of 4 * 9 * Cin / 64.  Each step commits its main and
 // its cross MMAs as two groups; the promotion waits for the main group only and overlaps the cross MMAs.
+// Epilogue handoff (PR = 0): the MMA warpgroups write a 64-channel half of the combined tile into the staging buffer and
+// arrive on epiF (256 arrivals); the epilogue warpgroup lifts its pixel's 64 channels into registers and arrives on epiE
+// (128 arrivals) before it converts and stores them, so the MMA warpgroups wait for one shared-memory pass per half.
 template <int BN, int P, int TAPS, int MC, int F8, int PR = 0>
-__global__ void __launch_bounds__(kTcThreads, 1)
+__global__ void __launch_bounds__(kTcThreads<BN, PR>, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const ConvTcParams p) {
   using namespace ptx;
   constexpr int kBBytes = BN * 128;
+  constexpr bool EW = kEpiWarpgroup<BN, PR>;
   static_assert(!F8 || P == 2, "F16F8 uses two stage slots per operand");
   static_assert(!PR || (P == 3 && !F8), "promotion is built for three bf16 planes");
   extern __shared__ uint8_t smem_raw[];
@@ -111,9 +293,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const uint32_t a_stage = (uint32_t)P * p.patch_bytes, b_stage = (uint32_t)P * kBBytes;
   const uint32_t ring_b = ring_a + (uint32_t)p.stages_a * a_stage;
   float *epi = reinterpret_cast<float *>(smem_raw + (ring_b - raw) + (size_t)p.stages_b * b_stage);
-  uint8_t *ctrl = reinterpret_cast<uint8_t *>(epi) + kEpiBytes;
+  uint4 *xpose = reinterpret_cast<uint4 *>(reinterpret_cast<uint8_t *>(epi) + kEpiBytes);   // EW: the transpose blocks
+  uint8_t *ctrl = reinterpret_cast<uint8_t *>(epi) + kEpiBytes + (EW ? kXposeBytes : 0);
   const uint32_t fullA = smem_u32(ctrl), emptyA = fullA + 8 * kMaxStages;
   const uint32_t fullB = emptyA + 8 * kMaxStages, emptyB = fullB + 8 * kMaxStages;
+  const uint32_t epiF = emptyB + 8 * kMaxStages, epiE = epiF + 8;
 
   // warp index through a shuffle so the compiler knows it is warp-uniform: the role loops below are executed by
   // whole warps with uniform control flow and only the instruction issue is predicated on one elected lane --
@@ -128,6 +312,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       mbar_init(fullB + 8 * s, 1);
       mbar_init(emptyB + 8 * s, MC ? 4 : 2);    // ... of each CTA of the cluster
     }
+    mbar_init(epiF, 256);
+    mbar_init(epiE, 128);
     fence_mbar_init();
   }
   __syncthreads();
@@ -145,8 +331,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   constexpr int halo = TAPS == 9 ? 1 : 0;
 
+  // registers (EW): 128 x 24 + 256 x 168 + 128 x 152 = the 65 536 of the SM
   if (warp < 4) {
-    regs_dealloc<40>();
+    if (EW) regs_dealloc<24>();
+    else regs_dealloc<40>();
     if (warp == 1) {
       // ===== activation (A) producer: one halo patch per plane per channel block =====
       int s = 0;
@@ -200,10 +388,43 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
+  } else if (EW && warp >= 12) {
+    regs_alloc<152>();
+    // ===== epilogue warpgroup: thread = pixel m of the tile; per 64-channel half, lift the pixel's two 32-channel chunks
+    // from the staging buffer, free the buffer, then convert and store them =====
+    const int m = (warp & 3) * 32 + lane;
+    uint4 *stage_w = xpose + (warp & 3) * 32;
+    uint32_t eph = 0;
+    if (!CTPN_DBG(p, 16)) {
+      for (int u = u_begin; u < p.total_units; u += u_step) {
+        int mt, nt;
+        unit_tile(u, mt, nt);
+        EpiPixel e;
+        epi_pixel(p, mt, m, lane, e);
+#pragma unroll 1
+        for (int c2 = 0; c2 < BN / 64; ++c2) {
+          float v[2][32];
+          mbar_wait(epiF, eph);
+#pragma unroll
+          for (int es = 0; es < 2; ++es) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const float4 t = *reinterpret_cast<const float4 *>(epi + es * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
+              v[es][4 * q + 0] = t.x; v[es][4 * q + 1] = t.y; v[es][4 * q + 2] = t.z; v[es][4 * q + 3] = t.w;
+            }
+          }
+          mbar_arrive(epiE);
+          eph ^= 1u;
+#pragma unroll
+          for (int es = 0; es < 2; ++es) epi_chunk<P, F8>(p, e, v[es], nt * BN + (2 * c2 + es) * 32, stage_w, true, false, lane);
+        }
+      }
+    }
   } else {
-    regs_alloc<232>();
-    // ===== consumers: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64) (pixel tile rows 8 wg .. 8 wg + 7) against all
-    // BN channels, then both warpgroups run the epilogue of the tile through a float32 staging buffer =====
+    if (EW) regs_alloc<168>();
+    else regs_alloc<232>();
+    // ===== MMA warpgroups: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64) (pixel tile rows 8 wg .. 8 wg + 7) against
+    // all BN channels, then hands the tile to the epilogue warpgroup (PR: runs the epilogue itself) =====
     const int wg = (warp >> 2) - 1;
     const bool leader = (threadIdx.x & 127) == 0;
     constexpr int R = BN / 2;                  // accumulator registers per thread (64 x BN per warpgroup)
@@ -220,14 +441,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     constexpr uint32_t kHiB = gmma_desc_hi(1024);
     const uint32_t hi_a = gmma_desc_hi((uint32_t)p.group_stride_bytes);
     const uint32_t wg_off = (uint32_t)wg * 8u * (uint32_t)p.group_stride_bytes;   // 8 row groups of 8 pixels per warpgroup
-    // epilogue geometry: consumer warp cw = set (even / odd 32-channel chunks) x quarter of the 128 pixels; thread = pixel m
-    const int cw = warp - 4, eset = cw >> 2, quarter = cw & 3;
-    const int m = quarter * 32 + lane;
-    const int th = m >> p.tw_log2, tw = m & (p.TW - 1);
-    const bool pool = (p.flags & CTPN_F_POOL) != 0, relu = (p.flags & CTPN_F_RELU) != 0;
-    const bool out_f32 = (p.flags & CTPN_F_OUT_F32) != 0;
     int sa = 0, sb = 0, prev_b = -1, prev_a = -1;
-    uint32_t pha = 0, phb = 0;
+    uint32_t pha = 0, phb = 0, eph = 0;
+    // accumulator fragments -> staging: 64 channels (fragments 8 c2 .. 8 c2 + 7) as two [128 pixels][32 channels] float32
+    // chunks, 16-byte pieces XOR-swizzled by pixel & 7
+    const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // accumulator fragment rows frow, frow + 8
+    auto stage_half = [&](int c2) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int i8 = c2 * 8 + j, q = 2 * (j & 3) + ((lane & 3) >> 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frow + 8 * h;
+          *reinterpret_cast<float2 *>(epi + (j >> 2) * 4096 + row * 32 + ((q ^ (row & 7)) << 2) + 2 * (lane & 1)) =
+              make_float2(accm[4 * i8 + 2 * h], accm[4 * i8 + 2 * h + 1]);
+        }
+      }
+    };
     // a weight stage (and after its last tap an activation stage) is released once the MMAs that read it have completed
     auto release = [&](int sbx, int sax) {
       if (leader) {
@@ -334,202 +564,54 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           accm[i] = F8 ? __fmaf_rn(accc[i], p.inv_cross, accm[i] * p.inv_main) : PR ? __fadd_rn(accs[i], accc[i]) : accm[i] + accc[i];
       }
 
-      // ===== epilogue: +bias -> ReLU -> optional fused 2x2 max-pool (warp shuffles: the window of a pixel lives in lanes
-      // l, l^1, l^8, l^9) -> re-split into planes -> transpose through swizzled shared memory -> 16-byte stores that cover
-      // one pixel's 64 contiguous bytes with 4 lanes (or float32 output) =====
-      int mt, nt;
-      unit_tile(u, mt, nt);
-      const int b = mt / tiles_per_img, r = mt % tiles_per_img;
-      const int y = (r / p.tiles_x) * p.TH + th, x = (r % p.tiles_x) * p.TW + tw;
-      bool ok, live = true;       // live = false: a pad row of a stacked frame (stored as zeros when the output is stacked)
-      int oy, ox, ob = b;
-      if (pool) {
-        oy = y >> 1; ox = x >> 1;
-        ok = !(th & 1) && !(tw & 1) && oy < p.Ho && ox < p.Wo;
-      } else {
-        oy = y; ox = x;
-        ok = y < p.H && x < p.W;
-        if (p.in_stack_h) {       // stacked input: y runs over the whole stack (the kernel sees one image of B * in_stack_h rows)
-          ob = y / p.in_stack_h;
-          oy = y - ob * p.in_stack_h;
-          live = oy < p.in_stack_h - 1;
-          if (!p.out_stacked) ok = ok && live;
-        }
-      }
-      if (p.ext) {     // ragged batch: zero outside the image's extent at the output level (with a pool: the whole window)
-        const int ib = min(ob, p.ext_n - 1);
-        live = live && oy < (__ldg(p.ext + 2 * ib) >> p.ext_shift) && ox < (__ldg(p.ext + 2 * ib + 1) >> p.ext_shift);
-      }
-      const long long pix = ((long long)ob * p.out_rows + oy) * p.Wo + ox;
-      // coalesced plane stores: the warp's 32-pixel x 32-channel block is transposed through shared memory so
-      // that 4 consecutive lanes write the 64 contiguous bytes of one pixel (full 32-B sectors) instead of every
-      // lane writing 16 B of its own pixel.  Lane l stores for pixels (l >> 2) + 8 * it, 16-byte chunk l & 3.
-      const unsigned okmask = __ballot_sync(0xffffffffu, ok);
-      long long spix[4];
+      if (CTPN_DBG(p, 16)) continue;
+      if (EW) {
+        // +bias -> ReLU here, where the thread's 2 x BN / 8 channels come with few loads, then hand the tile over in
+        // 64-channel halves; the epilogue warpgroup frees the buffer once it has read a half
+        const float *bt = p.bias + (u % p.tiles_n) * BN + 2 * (lane & 3);   // accm[4 i8 + 2 h + k]: channel 8 i8 + 2 (lane & 3) + k
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const long long hi = __shfl_sync(0xffffffffu, (int)(pix >> 32), it * 8 + (lane >> 2));
-        const unsigned lo = __shfl_sync(0xffffffffu, (unsigned)(pix & 0xffffffffll), it * 8 + (lane >> 2));
-        spix[it] = (hi << 32) | lo;
-      }
-      // float32 staging [2 chunks][128 pixels][32 channels], 16-byte chunks XOR-swizzled by pixel & 7; the 32 rows a warp
-      // reads back are its own, and once read they serve as its store-transpose block
-      uint4 *stage_w = reinterpret_cast<uint4 *>(epi + eset * 4096 + quarter * 1024);
-      const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // accumulator fragment rows frow, frow + 8
-      if (!CTPN_DBG(p, 16)) {
-#pragma unroll
-      for (int c2 = 0; c2 < BN / 64; ++c2) {
-        named_sync(1, 256);           // the previous chunk pair has been read
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int i8 = c2 * 8 + j, q = 2 * (j & 3) + ((lane & 3) >> 1);
+        for (int i8 = 0; i8 < BN / 8; ++i8) {
+          const float2 bq = __ldg(reinterpret_cast<const float2 *>(bt + 8 * i8));
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int row = frow + 8 * h;
-            *reinterpret_cast<float2 *>(epi + (j >> 2) * 4096 + row * 32 + ((q ^ (row & 7)) << 2) + 2 * (lane & 1)) =
-                make_float2(accm[4 * i8 + 2 * h], accm[4 * i8 + 2 * h + 1]);
+            accm[4 * i8 + 2 * h] += bq.x;
+            accm[4 * i8 + 2 * h + 1] += bq.y;
           }
         }
-        named_sync(1, 256);
-        const int chunk = 2 * c2 + eset;
-        const int c0 = nt * BN + chunk * 32;
-        float v[32];
+        if (p.flags & CTPN_F_RELU) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 t = *reinterpret_cast<const float4 *>(epi + eset * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
-          v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+          for (int i = 0; i < R; ++i) accm[i] = fmaxf(accm[i], 0.f);
         }
 #pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const float4 bq = __ldg(reinterpret_cast<const float4 *>(p.bias + c0) + q);
-          v[4 * q + 0] += bq.x;
-          v[4 * q + 1] += bq.y;
-          v[4 * q + 2] += bq.z;
-          v[4 * q + 3] += bq.w;
+        for (int c2 = 0; c2 < BN / 64; ++c2) {
+          mbar_wait(epiE, eph ^ 1u);
+          stage_half(c2);
+          mbar_arrive(epiF);
+          eph ^= 1u;
         }
-        if (relu) {
+      } else {
+        // both MMA warpgroups run the epilogue: warp cw = set (even / odd 32-channel chunks) x quarter of the 128 pixels
+        const int cw = warp - 4, eset = cw >> 2, quarter = cw & 3;
+        const int m = quarter * 32 + lane;
+        int mt, nt;
+        unit_tile(u, mt, nt);
+        EpiPixel e;
+        epi_pixel(p, mt, m, lane, e);
+        // the 32 staging rows a warp reads back are its own, and once read they serve as its store-transpose block
+        uint4 *stage_w = reinterpret_cast<uint4 *>(epi + eset * 4096 + quarter * 1024);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
+        for (int c2 = 0; c2 < BN / 64; ++c2) {
+          named_sync(1, 256);           // the previous chunk pair has been read
+          stage_half(c2);
+          named_sync(1, 256);
+          float v[32];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float4 t = *reinterpret_cast<const float4 *>(epi + eset * 4096 + m * 32 + ((q ^ (m & 7)) << 2));
+            v[4 * q + 0] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+          }
+          epi_chunk<P, F8>(p, e, v, nt * BN + (2 * c2 + eset) * 32, stage_w, false, true, lane);
         }
-        if (!live) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0.f;
-        }
-        if (pool) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            v[i] = fmaxf(v[i], __shfl_xor_sync(0xffffffffu, v[i], 1));
-            v[i] = fmaxf(v[i], __shfl_xor_sync(0xffffffffu, v[i], p.TW));
-          }
-        }
-        if (F8 && pool && !out_f32 && !(p.flags & CTPN_F_OUT_BF16X2)) {
-          // Pooled F16F8 output without staging: after the shuffles all four lanes of a 2x2 window (l, l^1, l^8, l^9) hold the
-          // pooled value, so each takes one quarter (8 channels) of the chunk: a quarter of the conversions, and the four
-          // lanes' stores form 64 contiguous bytes of the fp16 plane and 32 + 32 of the e4m3 plane (full sectors).
-          const int j = (lane & 1) | ((lane >> 2) & 2);
-          float x[8];
-#pragma unroll
-          for (int k = 0; k < 8; ++k) x[k] = j == 0 ? v[k] : j == 1 ? v[8 + k] : j == 2 ? v[16 + k] : v[24 + k];
-          const bool okw = oy < p.Ho && ox < p.Wo;     // (pix already points into the stacked frame when out_rows = Ho + 1)
-          uint4 hw;
-          uint2 qv, qr;
-          f16f8_quad(x[0], x[1], x[2], x[3], p.out_s, p.out_t, p.out_rs, hw.x, hw.y, qv.x, qr.x);
-          f16f8_quad(x[4], x[5], x[6], x[7], p.out_s, p.out_t, p.out_rs, hw.z, hw.w, qv.y, qr.y);
-          if (okw && c0 < p.Cout && !CTPN_DBG(p, 8)) {
-            uint8_t *o0 = reinterpret_cast<uint8_t *>(p.out) + pix * p.Cout * 2;
-            uint8_t *o1 = o0 + p.out_plane_stride * 2 + (long long)(c0 >> 6) * 128 + (c0 & 63) + j * 8;
-            *reinterpret_cast<uint4 *>(o0 + (long long)c0 * 2 + j * 16) = hw;
-            *reinterpret_cast<uint2 *>(o1) = qv;
-            *reinterpret_cast<uint2 *>(o1 + 64) = qr;
-          }
-        } else if (F8 && !out_f32 && !(p.flags & CTPN_F_OUT_BF16X2)) {
-          // F16F8 planes: fp16 words, then the e4m3 copies of the values and of the residuals (8 + 8 words)
-          uint32_t wh[16], wq[16];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            f16f8_quad(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3], p.out_s, p.out_t, p.out_rs, wh[2 * i], wh[2 * i + 1], wq[i], wq[8 + i]);
-          }
-          const int j = lane & 3;
-#pragma unroll
-          for (int pl = 0; pl < 2; ++pl) {
-            // plane 0: 64 contiguous bytes per pixel (32 fp16).  plane 1: the pixel's 128-byte block of channel block
-            // c0 / 64 holds values at +0 and residuals at +64; this chunk owns 32 bytes of each
-            uint8_t *obase = reinterpret_cast<uint8_t *>(p.out) + (long long)pl * p.out_plane_stride * 2;
-            const long long off = pl == 0 ? (long long)c0 * 2 + j * 16
-                                          : (long long)(c0 >> 6) * 128 + (c0 & 63) + (j >> 1) * 64 + (j & 1) * 16;
-            const bool st_ok = c0 < p.Cout && !CTPN_DBG(p, 8);
-            if (!p.stage_small) {
-              __syncwarp();     // previous readers of the staging block are done
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const uint4 val = pl == 0 ? make_uint4(wh[4 * q], wh[4 * q + 1], wh[4 * q + 2], wh[4 * q + 3])
-                                          : make_uint4(wq[4 * q], wq[4 * q + 1], wq[4 * q + 2], wq[4 * q + 3]);
-                stage_w[lane * 4 + (q ^ ((lane >> 1) & 3))] = val;
-              }
-              __syncwarp();
-              if (st_ok) {
-#pragma unroll
-                for (int it = 0; it < 4; ++it) {
-                  const int pp = it * 8 + (lane >> 2);
-                  const uint4 val = stage_w[pp * 4 + (j ^ ((pp >> 1) & 3))];
-                  if ((okmask >> pp) & 1u) *reinterpret_cast<uint4 *>(obase + spix[it] * p.Cout * 2 + off) = val;
-                }
-              }
-            } else {
-              // 8 pixels per round through a 512-byte block: lanes 8 it .. 8 it + 7 deposit their 64 bytes, all 32 lanes
-              // then store one 16-byte piece each (4 lanes = one pixel's 64 contiguous bytes)
-#pragma unroll
-              for (int it = 0; it < 4; ++it) {
-                __syncwarp();
-                if ((lane >> 3) == it) {
-                  const int row = lane & 7;
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) {
-                    const uint4 val = pl == 0 ? make_uint4(wh[4 * q], wh[4 * q + 1], wh[4 * q + 2], wh[4 * q + 3])
-                                              : make_uint4(wq[4 * q], wq[4 * q + 1], wq[4 * q + 2], wq[4 * q + 3]);
-                    stage_w[row * 4 + (q ^ ((row >> 1) & 3))] = val;
-                  }
-                }
-                __syncwarp();
-                const int row = lane >> 2, pp = it * 8 + row;
-                const uint4 val = stage_w[row * 4 + (j ^ ((row >> 1) & 3))];
-                if (st_ok && ((okmask >> pp) & 1u)) *reinterpret_cast<uint4 *>(obase + spix[it] * p.Cout * 2 + off) = val;
-              }
-            }
-          }
-        } else if (!out_f32) {
-          uint32_t w[P][16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            uint32_t t[P];
-            split_planes2<P>(v[2 * i], v[2 * i + 1], t);
-#pragma unroll
-            for (int pl = 0; pl < P; ++pl) w[pl][i] = t[pl];
-          }
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl) {
-            __syncwarp();     // previous readers of the staging block are done
-#pragma unroll
-            for (int q = 0; q < 4; ++q) stage_w[lane * 4 + (q ^ ((lane >> 1) & 3))] = make_uint4(w[pl][4 * q], w[pl][4 * q + 1], w[pl][4 * q + 2], w[pl][4 * q + 3]);
-            __syncwarp();
-            if (c0 < p.Cout && !CTPN_DBG(p, 8)) {
-              __nv_bfloat16 *obase = reinterpret_cast<__nv_bfloat16 *>(p.out) + (long long)pl * p.out_plane_stride + c0 + (lane & 3) * 8;
-#pragma unroll
-              for (int it = 0; it < 4; ++it) {
-                const int pp = it * 8 + (lane >> 2);
-                const uint4 val = stage_w[pp * 4 + ((lane & 3) ^ ((pp >> 1) & 3))];
-                if ((okmask >> pp) & 1u) *reinterpret_cast<uint4 *>(obase + spix[it] * p.Cout) = val;
-              }
-            }
-          }
-        } else if (ok && c0 < p.Cout && !CTPN_DBG(p, 8)) {
-          if (out_f32) {
-            float4 *dst = reinterpret_cast<float4 *>(reinterpret_cast<float *>(p.out) + pix * p.Cout + c0);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          }
-        }
-      }
       }
     }
   }
@@ -546,7 +628,7 @@ constexpr int kMaxDevices = 64;
 static std::mutex g_mu;
 static int g_sms[kMaxDevices];
 
-struct Tuning { int debug = 0, bn = 0, stages_a = 0, stages_b = 0, mcast = 1, stage_small = 1, promote = 1; };
+struct Tuning { int debug = 0, bn = 0, stages_a = 0, stages_b = 0, mcast = 1, promote = 1; };
 static const Tuning &tuning() {            // read once at first use; overrides exist only in the test library
   static const Tuning t = [] {
     Tuning v;
@@ -557,7 +639,6 @@ static const Tuning &tuning() {            // read once at first use; overrides 
     v.stages_a = env_int("CTPN_TC_STAGES_A", 0);
     v.stages_b = env_int("CTPN_TC_STAGES_B", 0);
     v.mcast = env_int("CTPN_TC_MCAST", 1);
-    v.stage_small = env_int("CTPN_TC_STAGE_SMALL", 1);
     v.promote = std::max(1, env_int("CTPN_TC_PROMOTE", 1));   // CTPN_F_PROMOTE: pipeline steps per promoted main chain
 #endif
     return v;
@@ -606,10 +687,8 @@ static int cached_tmap(int dev, CUtensorMap *out, const void *ptr, int rank, con
 template <int BN, int P, int TAPS, int MC, int F8 = 0, int PR = 0>
 static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, ConvTcParams &p, cudaStream_t st) {
   const size_t a_stage = (size_t)p.planes * p.patch_bytes, b_stage = (size_t)p.planes * BN * 128;
-  // long-K F16F8 layers store through 8-pixel rounds (a 512-byte transpose block per warp)
-  const bool small = F8 && TAPS == 9 && p.Cin >= 256 && !(p.flags & (CTPN_F_OUT_F32 | CTPN_F_OUT_BF16X2 | CTPN_F_POOL)) && tuning().stage_small != 0;
-  p.stage_small = small ? 1 : 0;
-  const size_t budget = 227 * 1024 - 1024 - kCtrlBytes - kEpiBytes;
+  const size_t epi_bytes = kEpiBytes + (kEpiWarpgroup<BN, PR> ? kXposeBytes : 0);     // staging (+ the epilogue warpgroup's transpose blocks)
+  const size_t budget = 227 * 1024 - 1024 - kCtrlBytes - epi_bytes;
   // activation ring: two stages when they leave room for at least two weight stages, else one
   int sa = (2 * a_stage + 2 * b_stage <= budget) ? 2 : 1;
   if (p.taps == 1) sa = (int)std::min<size_t>(4, std::max<size_t>(1, (budget / 2) / a_stage));
@@ -621,7 +700,7 @@ static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, Conv
   if (tuning().stages_b > 0) sb = std::max(2, std::min(sb, tuning().stages_b));
   p.stages_a = sa;
   p.stages_b = sb;
-  const size_t smem = 1024 + sa * a_stage + sb * b_stage + kEpiBytes + kCtrlBytes;
+  const size_t smem = 1024 + sa * a_stage + sb * b_stage + epi_bytes + kCtrlBytes;
   CTPN_REQUIRE(smem <= 227 * 1024, "conv_tc: %zu bytes of shared memory", smem);
   auto kernel = conv_tc_kernel<BN, P, TAPS, MC, F8, PR>;
   static bool attr_set[kMaxDevices];
@@ -630,7 +709,7 @@ static int launch_bn(int dev, const CUtensorMap &ta, const CUtensorMap &tb, Conv
   cudaLaunchAttribute attr;
   attr.id = cudaLaunchAttributeClusterDimension;
   attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-  cfg.blockDim = dim3(kTcThreads);
+  cfg.blockDim = dim3(kTcThreads<BN, PR>);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cfg.attrs = &attr;
