@@ -23,6 +23,7 @@
  *   ctpn_image_blob_f32     _get_image_blob, lib/fast_rcnn/test.py:7-31 (float32 cv2.resize of the mean-subtracted image)
  *   ctpn_resize_linear_u8_ragged / ctpn_image_blob_f32_ragged   the same two, for a batch of images of different sizes
  *   ctpn_resize_linear_u8_ragged_rows     the ragged resize on sources that hold only the rows it reads
+ *   ctpn_resize_linear_u8_strided         the ragged resize on images read in place at any byte strides
  *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host / ctpn_text_lines (batched, device)
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
@@ -256,6 +257,21 @@ int ctpn_resize_linear_u8_ragged_rows(const void *src, size_t src_elems, const l
                                       const int *stored_rows, const int *row_map, size_t map_elems, const long long *map_offset,
                                       const double *fxy, const int *dst_hw, int B, int channels, void *dst, int H, int W,
                                       void *stream);
+
+/* ctpn_resize_linear_u8_ragged for images read in place from memory the caller owns (e.g. device tensors of any strides):
+ * image b is the (h, w) = src_hw[2b..2b+1] uint8 image whose sample (y, x, c) lies at byte
+ *   src[b] + src_offset[b] + y * src_strides[3b] + x * src_strides[3b + 1] + c * src_strides[3b + 2]
+ * of the allocation src[b] (a DEVICE address) of src_bytes[b] bytes.  Strides are signed and may be zero, so channel
+ * order and planar layouts are strides too: an RGB image is read as BGR from channel 2 with a negative channel stride.
+ * The 3-channel output is written exactly as ctpn_resize_linear_u8_ragged writes it (rows < dh, columns < dw of slice b of
+ * dst [B][H][W][3]; the rest NOT written), bit-identical to it on a dense BGR copy of the image.  src, src_bytes,
+ * src_offset, src_strides, src_hw, fxy and dst_hw are HOST arrays (1 <= B <= 64).  Validated before any CUDA call, with
+ * the size, scale, dst_hw and canvas rules of ctpn_resize_linear_u8_ragged and in addition (CTPN_ERR_INVALID naming the
+ * image): a NULL src[b]; the lowest and the highest byte the h x w x 3 box can touch must lie in [0, src_bytes[b]); the
+ * column and channel strides must fit in 32 bits. */
+int ctpn_resize_linear_u8_strided(const void *const *src, const size_t *src_bytes, const long long *src_offset,
+                                  const long long *src_strides, const int *src_hw, const double *fxy, const int *dst_hw, int B,
+                                  void *dst, int H, int W, void *stream);
 
 /* CRC-32C (Castagnoli) of a host buffer, continuing from `crc` (0 to start): the per-tensor checksum of TF checkpoint V2
  * files, used by the weight importer (ctpn_b200/tf_import.py) to verify every tensor it loads. */

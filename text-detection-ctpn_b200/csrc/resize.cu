@@ -19,7 +19,8 @@
 //
 // The *_ragged entry points run both for a batch of images of different sizes (Engine.rois_images); they share the
 // per-pixel functions below with the single-image kernels.  ctpn_resize_linear_u8_ragged_rows is the ragged resize on
-// sources that hold only the rows it reads (Engine.stream_rois_images uploads camera photos that way).
+// sources that hold only the rows it reads (Engine.stream_rois_images uploads camera photos that way), and
+// ctpn_resize_linear_u8_strided the ragged resize on images read in place at any byte strides (CUDA tensors of callers).
 #include "common.cuh"
 
 namespace ctpn {
@@ -39,33 +40,54 @@ __device__ __forceinline__ void resize_taps(int d, int sn, double scale, bool dr
   s1 = min(max(s + 1, 0), sn - 1);
 }
 
-// Where source row y of an image is stored: every row in place ...
+// Where sample (y, x, c) of a source image is stored.  An accessor gives the start of row y (row) and the sample at
+// column x, channel c of such a row (at).  Interleaved [h][pitch][C] images with every row in place ...
 struct DenseRows {
-  __device__ __forceinline__ int operator()(int y) const { return y; }
+  const uint8_t *__restrict__ im;
+  int pitch, C;
+  __device__ __forceinline__ const uint8_t *row(int y) const { return im + (size_t)y * pitch * C; }
+  __device__ __forceinline__ uint8_t at(const uint8_t *r, int x, int c) const { return r[(size_t)x * C + c]; }
 };
 // ... or only the rows the resize reads (ctpn_resize_linear_u8_ragged_rows): map[y] is the stored index of source row y.
 // The map is device memory the host never saw, so the index is clamped to the stored extent the host did check.
 struct CompactRows {
+  const uint8_t *__restrict__ im;
+  int pitch, C;
   const int *__restrict__ map;
   int stored;
-  __device__ __forceinline__ int operator()(int y) const { return min(max(__ldg(map + y), 0), stored - 1); }
+  __device__ __forceinline__ const uint8_t *row(int y) const {
+    return im + (size_t)min(max(__ldg(map + y), 0), stored - 1) * pitch * C;
+  }
+  __device__ __forceinline__ uint8_t at(const uint8_t *r, int x, int c) const { return r[(size_t)x * C + c]; }
+};
+// ... or anywhere, at signed byte strides per row, column and channel (ctpn_resize_linear_u8_strided: a caller's device
+// tensor read in place; a negative channel stride from channel 2 reads RGB as BGR, a zero stride broadcasts).
+struct StridedPixels {
+  const uint8_t *base;         // sample (0, 0, 0)
+  long long row_stride;
+  int col_stride, chan_stride;
+  __device__ __forceinline__ const uint8_t *row(int y) const { return base + (long long)y * row_stride; }
+  __device__ __forceinline__ uint8_t at(const uint8_t *r, int x, int c) const {
+    return __ldg(r + ((long long)x * col_stride + (long long)c * chan_stride));
+  }
 };
 
-// One output pixel of cv2.resize(INTER_LINEAR) of a uint8 image im [sh][pitch][C] (pitch >= sw pixels per row) -> o[C].
-// Shared by the uniform and the ragged kernels: the ragged batch is bit-identical to single-image runs by construction.
-// Taps, weights and border clamping come from the source geometry (sh, sw); only the address of a row goes through
-// `row`.
-template <class Rows>
-__device__ __forceinline__ void resize_u8_pixel(const uint8_t *__restrict__ im, int sh, int sw, int pitch, int C, int dx, int dy,
-                                                double scale_x, double scale_y, bool area2, uint8_t *__restrict__ o,
-                                                const Rows row) {
+// One output pixel of cv2.resize(INTER_LINEAR) of a uint8 image of sh x sw pixels and C channels -> o[C].  Shared by
+// every uint8 resize kernel: a ragged or strided batch is bit-identical to single-image runs by construction.  Taps,
+// weights, the INTER_AREA route and rounding come from the source geometry (sh, sw); only the address of a sample goes
+// through the accessor `src`.
+template <class Src>
+__device__ __forceinline__ void resize_u8_pixel(const Src src, int sh, int sw, int C, int dx, int dy, double scale_x,
+                                                double scale_y, bool area2, uint8_t *__restrict__ o) {
   if (area2) {
     const int y0 = 2 * dy, x0 = 2 * dx;
     const int ny = min(2, sh - y0), nx = min(2, sw - x0);
     for (int c = 0; c < C; ++c) {
       int sum = 0;
-      for (int yy = 0; yy < ny; ++yy)
-        for (int xx = 0; xx < nx; ++xx) sum += im[((size_t)row(y0 + yy) * pitch + x0 + xx) * C + c];
+      for (int yy = 0; yy < ny; ++yy) {
+        const uint8_t *r = src.row(y0 + yy);
+        for (int xx = 0; xx < nx; ++xx) sum += src.at(r, x0 + xx, c);
+      }
       int v = (ny * nx == 4) ? (sum + 2) >> 2 : __float2int_rn(__fdiv_rn((float)sum, (float)(ny * nx)));
       o[c] = (uint8_t)min(max(v, 0), 255);
     }
@@ -74,10 +96,10 @@ __device__ __forceinline__ void resize_u8_pixel(const uint8_t *__restrict__ im, 
   int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
   resize_taps(dx, sw, scale_x, true, sx0, sx1, a0, a1);
   resize_taps(dy, sh, scale_y, false, sy0, sy1, b0, b1);
-  const uint8_t *r0 = im + (size_t)row(sy0) * pitch * C, *r1 = im + (size_t)row(sy1) * pitch * C;
+  const uint8_t *r0 = src.row(sy0), *r1 = src.row(sy1);
   for (int c = 0; c < C; ++c) {
-    const int h0 = r0[(size_t)sx0 * C + c] * a0 + r0[(size_t)sx1 * C + c] * a1;
-    const int h1 = r1[(size_t)sx0 * C + c] * a0 + r1[(size_t)sx1 * C + c] * a1;
+    const int h0 = src.at(r0, sx0, c) * a0 + src.at(r0, sx1, c) * a1;
+    const int h1 = src.at(r1, sx0, c) * a0 + src.at(r1, sx1, c) * a1;
     const int v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
     o[c] = (uint8_t)min(max(v, 0), 255);
   }
@@ -89,8 +111,8 @@ resize_linear_u8_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ d
   const long long total = (long long)B * dh * dw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int dx = (int)(i % dw), dy = (int)((i / dw) % dh), b = (int)(i / ((long long)dw * dh));
-    resize_u8_pixel(src + (size_t)b * sh * sw * C, sh, sw, sw, C, dx, dy, scale_x, scale_y, area2 != 0, dst + (size_t)i * C,
-                    DenseRows());
+    resize_u8_pixel(DenseRows{src + (size_t)b * sh * sw * C, sw, C}, sh, sw, C, dx, dy, scale_x, scale_y, area2 != 0,
+                    dst + (size_t)i * C);
   }
 }
 
@@ -174,8 +196,8 @@ __global__ void __launch_bounds__(256) resize_linear_u8_ragged_kernel(const uint
   const long long total = (long long)dh * dw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int dx = (int)(i % dw), dy = (int)(i / dw);
-    resize_u8_pixel(im, p.sh[b], p.sw[b], p.pitch[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
-                    out + ((size_t)dy * p.W + dx) * C, DenseRows());
+    resize_u8_pixel(DenseRows{im, p.pitch[b], C}, p.sh[b], p.sw[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
+                    out + ((size_t)dy * p.W + dx) * C);
   }
 }
 
@@ -193,13 +215,41 @@ __global__ void __launch_bounds__(256) resize_linear_u8_ragged_rows_kernel(const
   const RaggedResize &p = q.r;
   const int b = blockIdx.y, dh = p.dh[b], dw = p.dw[b], C = p.C;
   const uint8_t *im = src + p.src_offset[b];
-  const CompactRows row{rows + q.map_offset[b], q.stored[b]};
+  const CompactRows src_b{im, p.pitch[b], C, rows + q.map_offset[b], q.stored[b]};
   uint8_t *out = dst + (size_t)b * p.H * p.W * C;
   const long long total = (long long)dh * dw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int dx = (int)(i % dw), dy = (int)(i / dw);
-    resize_u8_pixel(im, p.sh[b], p.sw[b], p.pitch[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
-                    out + ((size_t)dy * p.W + dx) * C, row);
+    resize_u8_pixel(src_b, p.sh[b], p.sw[b], C, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
+                    out + ((size_t)dy * p.W + dx) * C);
+  }
+}
+
+// Images read in place at byte strides of their own (ctpn_resize_linear_u8_strided), written as the dense ragged kernel
+// writes them: 3 channels, canvas [B][H][W][3].  56 bytes per image, 3600 in all: with the dst pointer the kernel's
+// parameters stay within the 4 KB every CUDA 12 driver accepts, so the column and channel strides are 32-bit (the host
+// checks that they fit).
+struct StridedResize {
+  const uint8_t *base[kRaggedMax];     // sample (0, 0, 0) of image b
+  long long row_stride[kRaggedMax];
+  int col_stride[kRaggedMax], chan_stride[kRaggedMax];
+  double scale_x[kRaggedMax], scale_y[kRaggedMax];
+  int sh[kRaggedMax], sw[kRaggedMax], dh[kRaggedMax], dw[kRaggedMax];
+  unsigned long long area2;            // bit b: exact 1/2 in both directions
+  int H, W;
+};
+static_assert(sizeof(StridedResize) + sizeof(void *) <= 4096, "strided resize parameters exceed 4 KB");
+
+__global__ void __launch_bounds__(256) resize_linear_u8_strided_kernel(uint8_t *__restrict__ dst,
+                                                                       const __grid_constant__ StridedResize p) {
+  const int b = blockIdx.y, dh = p.dh[b], dw = p.dw[b];
+  const StridedPixels src_b{p.base[b], p.row_stride[b], p.col_stride[b], p.chan_stride[b]};
+  uint8_t *out = dst + (size_t)b * p.H * p.W * 3;
+  const long long total = (long long)dh * dw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int dx = (int)(i % dw), dy = (int)(i / dw);
+    resize_u8_pixel(src_b, p.sh[b], p.sw[b], 3, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
+                    out + ((size_t)dy * p.W + dx) * 3);
   }
 }
 
@@ -272,6 +322,23 @@ extern "C" int ctpn_image_blob_f32(const void *src_u8, const float *lut, int B, 
   return CTPN_OK;
 }
 
+// The per-image geometry rules of every ragged call: source size and scales, then the output size cv2 would produce,
+// which dst_hw must give and the canvas must hold.
+static int ragged_geometry_ok(const char *fn, int b, int sh, int sw, double fx, double fy, const int *dst_hw, int H, int W,
+                              int *eh, int *ew) {
+  CTPN_REQUIRE(sh > 0 && sw > 0, "%s: image %d: bad source size %d x %d", fn, b, sh, sw);
+  CTPN_REQUIRE(fx > 0 && fy > 0, "%s: image %d: scale (%g, %g) must be > 0", fn, b, fx, fy);
+  CTPN_REQUIRE(sh * fy < 1e9 && sw * fx < 1e9, "%s: image %d: scale (%g, %g) too large", fn, b, fx, fy);
+  if (ctpn_resize_out_size(sh, sw, fx, fy, eh, ew)) {
+    set_error("%s: image %d: %d x %d at (%g, %g) resizes to nothing", fn, b, sh, sw, fx, fy);
+    return CTPN_ERR_INVALID;
+  }
+  CTPN_REQUIRE(*eh == dst_hw[2 * b] && *ew == dst_hw[2 * b + 1], "%s: image %d: dst is %d x %d, cv2 would produce %d x %d", fn,
+               b, dst_hw[2 * b], dst_hw[2 * b + 1], *eh, *ew);
+  CTPN_REQUIRE(*eh <= H && *ew <= W, "%s: image %d: output %d x %d does not fit the %d x %d canvas", fn, b, *eh, *ew, H, W);
+  return CTPN_OK;
+}
+
 // Validates the per-image host descriptors of a ragged call and fills the kernel's parameter struct; no CUDA call.
 // stored (NULL: every row): how many of image b's rows the source holds (row-compacted sources).
 static int ragged_params(const char *fn, size_t src_elems, const long long *src_offset, const int *src_hwp, const double *fxy,
@@ -291,8 +358,6 @@ static int ragged_params(const char *fn, size_t src_elems, const long long *src_
     const long long off = src_offset[b];
     CTPN_REQUIRE(sh > 0 && sw > 0, "%s: image %d: bad source size %d x %d", fn, b, sh, sw);
     CTPN_REQUIRE(pitch >= sw, "%s: image %d: row pitch %d < width %d", fn, b, pitch, sw);
-    CTPN_REQUIRE(fx > 0 && fy > 0, "%s: image %d: scale (%g, %g) must be > 0", fn, b, fx, fy);
-    CTPN_REQUIRE(sh * fy < 1e9 && sw * fx < 1e9, "%s: image %d: scale (%g, %g) too large", fn, b, fx, fy);
     CTPN_REQUIRE(off >= 0, "%s: image %d: negative source offset %lld", fn, b, off);
     const int held = stored ? stored[b] : sh;
     CTPN_REQUIRE(held >= 1 && held <= sh, "%s: image %d: %d stored rows, must be 1..%d (the source height)", fn, b, held, sh);
@@ -301,13 +366,8 @@ static int ragged_params(const char *fn, size_t src_elems, const long long *src_
     CTPN_REQUIRE(end <= (unsigned __int128)src_elems, "%s: image %d: source extent ends at %llu, past src_elems = %zu", fn, b,
                  (unsigned long long)end, src_elems);
     int eh = 0, ew = 0;
-    if (ctpn_resize_out_size(sh, sw, fx, fy, &eh, &ew)) {
-      set_error("%s: image %d: %d x %d at (%g, %g) resizes to nothing", fn, b, sh, sw, fx, fy);
-      return CTPN_ERR_INVALID;
-    }
-    CTPN_REQUIRE(eh == dst_hw[2 * b] && ew == dst_hw[2 * b + 1], "%s: image %d: dst is %d x %d, cv2 would produce %d x %d", fn, b,
-                 dst_hw[2 * b], dst_hw[2 * b + 1], eh, ew);
-    CTPN_REQUIRE(eh <= H && ew <= W, "%s: image %d: output %d x %d does not fit the %d x %d canvas", fn, b, eh, ew, H, W);
+    const int rc = ragged_geometry_ok(fn, b, sh, sw, fx, fy, dst_hw, H, W, &eh, &ew);
+    if (rc) return rc;
     p->src_offset[b] = off;
     p->sh[b] = sh;
     p->sw[b] = sw;
@@ -393,6 +453,63 @@ extern "C" int ctpn_image_blob_f32_ragged(const void *src_u8, size_t src_elems, 
   for (int b = 0; b < B; ++b) work += (long long)p.dh[b] * p.dw[b] * 3;
   ProfScope prof("image_blob_f32_ragged", (double)work, (cudaStream_t)stream);
   image_blob_f32_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const uint8_t *)src_u8, lut, dst, p);
+  CTPN_LAUNCH_CHECK();
+  return CTPN_OK;
+}
+
+extern "C" int ctpn_resize_linear_u8_strided(const void *const *src, const size_t *src_bytes, const long long *src_offset,
+                                             const long long *src_strides, const int *src_hw, const double *fxy,
+                                             const int *dst_hw, int B, void *dst, int H, int W, void *stream) {
+  const char *fn = "ctpn_resize_linear_u8_strided";
+  CTPN_REQUIRE(dst, "%s: null pointer", fn);
+  CTPN_REQUIRE(src && src_bytes && src_offset && src_strides && src_hw && fxy && dst_hw, "%s: null descriptor array", fn);
+  CTPN_REQUIRE(B >= 1 && B <= kRaggedMax, "%s: B = %d, must be 1..%d", fn, B, kRaggedMax);
+  CTPN_REQUIRE(H > 0 && W > 0, "%s: bad canvas %d x %d", fn, H, W);
+  StridedResize p;
+  memset(&p, 0, sizeof(p));
+  p.H = H;
+  p.W = W;
+  long long max_pixels = 0, work = 0;
+  for (int b = 0; b < B; ++b) {
+    const int sh = src_hw[2 * b], sw = src_hw[2 * b + 1];
+    CTPN_REQUIRE(src[b], "%s: image %d: null source", fn, b);
+    CTPN_REQUIRE(sh > 0 && sw > 0, "%s: image %d: bad source size %d x %d", fn, b, sh, sw);
+    const long long off = src_offset[b], *st = src_strides + 3 * b;
+    CTPN_REQUIRE(st[1] >= INT_MIN && st[1] <= INT_MAX && st[2] >= INT_MIN && st[2] <= INT_MAX,
+                 "%s: image %d: column / channel stride (%lld, %lld) outside the 32-bit range", fn, b, st[1], st[2]);
+    // lowest and highest byte of the h x w x 3 box, relative to the allocation; 128-bit, so no stride can wrap them
+    __int128 lo = off, hi = off;
+    const long long extent[3] = {sh - 1, sw - 1, 2};
+    for (int d = 0; d < 3; ++d) {
+      const __int128 span = (__int128)extent[d] * st[d];
+      (span < 0 ? lo : hi) += span;
+    }
+    CTPN_REQUIRE(lo >= 0 && hi < (__int128)src_bytes[b],
+                 "%s: image %d: the box spans bytes [%lld, %lld] of its allocation, outside [0, %zu)", fn, b,
+                 (long long)std::max<__int128>(std::min<__int128>(lo, LLONG_MAX), LLONG_MIN),
+                 (long long)std::max<__int128>(std::min<__int128>(hi, LLONG_MAX), LLONG_MIN), src_bytes[b]);
+    int eh = 0, ew = 0;
+    const int rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew);
+    if (rc) return rc;
+    p.base[b] = (const uint8_t *)src[b] + off;
+    p.row_stride[b] = st[0];
+    p.col_stride[b] = (int)st[1];
+    p.chan_stride[b] = (int)st[2];
+    p.sh[b] = sh;
+    p.sw[b] = sw;
+    p.dh[b] = eh;
+    p.dw[b] = ew;
+    p.scale_x[b] = 1.0 / fxy[2 * b];
+    p.scale_y[b] = 1.0 / fxy[2 * b + 1];
+    if (p.scale_x[b] == 2.0 && p.scale_y[b] == 2.0) p.area2 |= 1ull << b;
+    max_pixels = std::max(max_pixels, (long long)eh * ew);
+    work += (long long)eh * ew * 3;
+  }
+  dim3 grid;
+  int rc = ragged_grid(B, max_pixels, &grid);
+  if (rc) return rc;
+  ProfScope prof("resize_linear_u8_strided", (double)work, (cudaStream_t)stream);
+  resize_linear_u8_strided_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint8_t *)dst, p);
   CTPN_LAUNCH_CHECK();
   return CTPN_OK;
 }

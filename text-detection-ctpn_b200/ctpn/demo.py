@@ -11,7 +11,12 @@ and the blob on the GPU as well (Engine.rois_images, ctpn_batch_device); the out
 --device-lines (with --device-frontend) builds the text lines on the GPU too (Engine.detect_lines_images): the files equal
 those of --device-frontend --native-connector.  --stream (with --device-frontend) reads and decodes the files one at a
 time while earlier ones are uploaded and computed (Engine.stream_rois_images / stream_lines_images, ctpn_stream_device);
-the output files are the same.
+the output files are the same.  --gpu-decode (with --device-frontend) decodes the JPEG files on the GPU
+(torchvision.io.decode_jpeg, nvJPEG) and passes the RGB tensors to the same calls, which read them in place: only the
+compressed files cross the bus.  nvJPEG's pixels are not cv2.imread's (another IDCT and chroma upsampling), so the files
+written equal those of --device-frontend on the decoded pixels, not on cv2's.  Files nvJPEG cannot stand in for -- not
+JPEG, an EXIF orientation other than 1 (cv2.imread rotates those), or a frame other than baseline or progressive
+Huffman with 1 or 3 components -- are read with cv2.imread and uploaded instead.
 """
 from __future__ import print_function
 
@@ -39,6 +44,7 @@ from lib.text_connector.text_connect_cfg import Config as TextLineCfg, native_cf
 RESULTS_DIR = "data/results"
 NATIVE_CONNECTOR = False      # --native-connector: C++ text-line connector of the library instead of the Python one
 DEVICE_LINES = False          # --device-lines: the library's device connector on each batch's rois (Engine.detect_lines_images)
+GPU_DECODE = False            # --gpu-decode: JPEG files decoded on the GPU (nvJPEG through torchvision), read in place
 
 
 def resize_im(im, scale, max_scale=None):
@@ -105,22 +111,95 @@ def ctpn_batch(sess, image_names):
     print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
 
 
+def jpeg_on_gpu(data):
+    """Whether nvJPEG's decode of the file `data` (bytes) stands in for cv2.imread's, judged from its markers alone: a JPEG
+    whose frame is baseline (SOF0) or progressive (SOF2) Huffman with 1 or 3 components, and whose EXIF orientation, if it
+    has one, is 1 (cv2.imread rotates the others; the CUDA decode does not)."""
+    if data[:2] != b"\xff\xd8":
+        return False
+    i, frame = 2, None
+    while i + 4 <= len(data) and frame is None:
+        if data[i] != 0xFF:
+            return False
+        marker = data[i + 1]
+        if marker == 0xFF:                     # fill byte
+            i += 1
+            continue
+        n = int.from_bytes(data[i + 2:i + 4], "big")
+        seg = data[i + 4:i + 2 + n]
+        if marker == 0xE1 and seg[:6] == b"Exif\x00\x00" and exif_orientation(seg[6:]) not in (None, 1):
+            return False
+        if 0xC0 <= marker <= 0xCF and marker not in (0xC4, 0xC8, 0xCC):     # SOFn (C4 DHT, C8 JPG, CC DAC are not frames)
+            frame = (marker, seg[5] if len(seg) > 5 else 0)
+        if marker == 0xDA:                     # scan before any frame
+            return False
+        i += 2 + n
+    return frame is not None and frame[0] in (0xC0, 0xC2) and frame[1] in (1, 3)
+
+
+def exif_orientation(tiff):
+    """The Orientation tag (0x0112) of IFD0 of an EXIF TIFF block, or None."""
+    if len(tiff) < 8 or tiff[:2] not in (b"II", b"MM"):
+        return None
+    order = "little" if tiff[:2] == b"II" else "big"
+    ifd = int.from_bytes(tiff[4:8], order)
+    if ifd + 2 > len(tiff):
+        return None
+    for k in range(int.from_bytes(tiff[ifd:ifd + 2], order)):
+        e = tiff[ifd + 2 + 12 * k:ifd + 14 + 12 * k]
+        if len(e) == 12 and int.from_bytes(e[:2], order) == 0x0112:
+            return int.from_bytes(e[8:10], order)
+    return None
+
+
+def read_on_device(names):
+    """The files as CUDA uint8 [H, W, 3] RGB tensors: JPEGs nvJPEG can stand in for decoded on the GPU in one batched call
+    (ImageReadMode.RGB: cv2.imread makes three channels of a grayscale JPEG too), every other file read by cv2.imread,
+    flipped to RGB on the host and uploaded, so that the engine's call takes device tensors only."""
+    import torch
+    from torchvision.io import ImageReadMode, decode_jpeg
+    datas = []
+    for name in names:
+        with open(name, "rb") as f:
+            datas.append(f.read())
+    gpu = [i for i, d in enumerate(datas) if jpeg_on_gpu(d)]
+    out = [None] * len(names)
+    if gpu:
+        decoded = decode_jpeg([torch.frombuffer(bytearray(datas[i]), dtype=torch.uint8) for i in gpu], mode=ImageReadMode.RGB,
+                              device="cuda")
+        for i, t in zip(gpu, decoded):
+            out[i] = t.permute(1, 2, 0)
+    for i, name in enumerate(names):
+        if out[i] is None:
+            out[i] = torch.from_numpy(np.ascontiguousarray(cv2.imread(name)[:, :, ::-1])).cuda()
+    return out
+
+
+def read_images(names):
+    """The images of a batch and their channel order: cv2.imread's BGR arrays, or with --gpu-decode RGB device tensors."""
+    if GPU_DECODE:
+        return read_on_device(names), "RGB"
+    return [cv2.imread(name) for name in names], "BGR"
+
+
 def ctpn_batch_device(sess, image_names):
-    """ctpn_batch with resize_im and _get_image_blob on the device (Engine.rois_images): the images go up as read, and
-    the resized images come back for draw_boxes.  Same TextDetector, draw_boxes and output files per image."""
+    """ctpn_batch with resize_im and _get_image_blob on the device (Engine.rois_images): the images go up as read (or are
+    decoded on the device with --gpu-decode), and the resized images come back for draw_boxes.  Same TextDetector,
+    draw_boxes and output files per image."""
     timer = Timer()
     timer.tic()
-    imgs = [cv2.imread(name) for name in image_names]
+    imgs, channels = read_images(image_names)
     if DEVICE_LINES:        # the lines of TextDetector(native=True), built on the device; only they come back with the images
         res = sess.engine.detect_lines_images(imgs, mode=cfg.TEST.DETECT_MODE, return_resized=True, scale=TextLineCfg.SCALE,
-                                              max_scale=TextLineCfg.MAX_SCALE, cfg=native_cfg())
+                                              max_scale=TextLineCfg.MAX_SCALE, cfg=native_cfg(), channels=channels)
         for name, (boxes, scale, img) in zip(image_names, res):
             draw_boxes(img, name, boxes, scale)
             print('{:s}: {:d} text lines'.format(name, boxes.shape[0]))
         timer.toc()
         print(('Detection of {:d} images took {:.3f}s').format(len(image_names), timer.total_time))
         return
-    res = sess.engine.rois_images(imgs, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
+    res = sess.engine.rois_images(imgs, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE,
+                                  channels=channels)
     for name, (r, im_scale, scale, img) in zip(image_names, res):
         scores, boxes = r[:, 0], r[:, 1:5] / np.float64(im_scale)      # the float64 division of test_ctpn
         textdetector = TextDetector(native=NATIVE_CONNECTOR)
@@ -137,8 +216,9 @@ def ctpn_stream_device(sess, image_names, batch):
     written when its result arrives, while later images are still on their way."""
     timer = Timer()
     timer.tic()
-    decoded = (cv2.imread(name) for name in image_names)
-    kw = dict(max_batch=batch, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE)
+    decoded = (read_images([name])[0][0] for name in image_names)
+    kw = dict(max_batch=batch, return_resized=True, scale=TextLineCfg.SCALE, max_scale=TextLineCfg.MAX_SCALE,
+              channels="RGB" if GPU_DECODE else "BGR")
     if DEVICE_LINES:
         results = sess.engine.stream_lines_images(decoded, mode=cfg.TEST.DETECT_MODE, cfg=native_cfg(), **kw)
     else:
@@ -177,6 +257,11 @@ def main(argv=None):
     ap.add_argument("--stream", action="store_true",
                     help="with --device-frontend: decode the files lazily and overlap decoding, upload and compute "
                          "(Engine.stream_rois_images / stream_lines_images); same output files")
+    ap.add_argument("--gpu-decode", action="store_true",
+                    help="with --device-frontend: decode JPEG files on the GPU (torchvision nvJPEG; lazily, one file at a time, "
+                         "with --stream) and read them in place.  nvJPEG's pixels differ from cv2.imread's, so the files equal "
+                         "those of --device-frontend on the decoded pixels, not on cv2's.  Other files, and JPEGs with an EXIF "
+                         "rotation or an unusual frame, are read with cv2 and uploaded")
     args = ap.parse_args(argv)
     if args.stream and not args.device_frontend:
         ap.error("--stream needs --device-frontend (and --batch N with N > 1)")
@@ -184,9 +269,12 @@ def main(argv=None):
         ap.error("--device-frontend needs --batch N with N > 1")
     if args.device_lines and not args.device_frontend:
         ap.error("--device-lines needs --device-frontend (and --batch N with N > 1)")
-    global NATIVE_CONNECTOR, DEVICE_LINES
+    if args.gpu_decode and not args.device_frontend:
+        ap.error("--gpu-decode needs --device-frontend (and --batch N with N > 1)")
+    global NATIVE_CONNECTOR, DEVICE_LINES, GPU_DECODE
     NATIVE_CONNECTOR = args.native_connector
     DEVICE_LINES = args.device_lines
+    GPU_DECODE = args.gpu_decode
     if os.path.exists(RESULTS_DIR):
         shutil.rmtree(RESULTS_DIR)
     os.makedirs(RESULTS_DIR)

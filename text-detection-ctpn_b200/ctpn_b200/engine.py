@@ -657,7 +657,7 @@ class Engine:
         resized = images if f == 1.0 else self.resize_images(images, f)
         return self.detect_batch(resized), f
 
-    def rois_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200):
+    def rois_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, channels="BGR"):
         """The front half of ctpn() (demo.py:59-61) plus test_ctpn for a list of raw HxWx3 uint8 BGR images of any sizes,
         front-end on the device: resize_im (short side -> scale, long side <= max_scale; resize=False: the images are
         already at that scale) and _get_image_blob (uint8 when im_scale == 1, else the mean-subtracted float32 rescale),
@@ -667,41 +667,43 @@ class Engine:
         extents.  Returns, in input order, (rois float32 [n,5] in blob coordinates, im_scale, f) per image -- and the
         resize_im output as a host uint8 array as a 4th item with return_resized (what draw_boxes draws on).  Every image
         is bit-identical to the host front-end with OpenCV's own code (IPP-dispatching cv2 builds differ on float
-        rescales) followed by detect on that image alone.  Raises ValueError on a bad image (see frontend_plan)."""
+        rescales) followed by detect on that image alone.  Raises ValueError on a bad image (see frontend_plan).
+
+        The images may instead all be CUDA uint8 [H, W, 3] tensors on this engine's device, at any strides (crop views,
+        chw.permute(1, 2, 0), zero strides): ctpn_resize_linear_u8_strided reads them in place, so no image crosses the
+        bus, and the results equal those of the same call on host copies.  They must be ready on the stream that is current
+        when the call is made (torch's rule); the engine synchronises nothing for them.  A list that mixes host images and
+        CUDA tensors, or a tensor on another device, raises ValueError before any device work.  channels="RGB": every image
+        of the call holds RGB (as torchvision decodes it) -- host images are flipped inside the packing copy, tensors are
+        read through a negative channel stride."""
         out = [None] * len(images)
         rows = self.result_rows()
         for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
-                                                                "rois_images"):
+                                                                "rois_images", channels=channels):
             for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, len(idxs), rows))):
                 out[i] = (r, items[k].im_scale, items[k].f) + ((resized[k],) if return_resized else ())
         return out
 
-    def _images_batches(self, images, resize, max_batch, return_resized, scale, max_scale, what, after=None):
+    def _images_batches(self, images, resize, max_batch, return_resized, scale, max_scale, what, after=None, channels="BGR"):
         """The batches of rois_images / detect_lines_images.  Per ragged batch: front-end, network and proposal layer on the
         device (detect_packed's buffer), then after(packed, items) -- device work enqueued on the rois, returning the buffer
         to bring back (None: the packed rois themselves) -- and one D2H of that buffer.  Yields (input indices, their
-        FrontendSteps, the pinned host copy, the resize_im outputs or None); the pinned copy is reused by the next batch."""
+        FrontendSteps, the pinned host copy, the resize_im outputs or None); the pinned copy is reused by the next batch.
+        Host images go up in one pinned H2D per batch; CUDA tensors (images_on_device) are read in place by
+        ctpn_resize_linear_u8_strided."""
         if not 1 <= int(max_batch) <= 64:
             raise ValueError("%s: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)" % what)
-        images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
+        check_channels(channels, what)
+        images = list(images)
+        device_images = images_on_device(images, self.device, what)
+        if not device_images:
+            images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
         plan = frontend_plan(images, resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg)
         lut = self._mean_lut()
         stream = N.stream_ptr()
         for idxs, (H, W) in ragged_plan([p.blob for p in plan], [p.dtype for p in plan], max_batch):
             B = len(idxs)
             items = [plan[i] for i in idxs]
-            nbytes = [images[i].size for i in idxs]
-            offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
-            total = int(sum(nbytes))
-            pinned = self._pin("frontend_src", (1 << max(20, (total - 1).bit_length()),), torch.uint8)   # grow-only sizes
-            pn = pinned.numpy()
-            for k, i in enumerate(idxs):
-                h, w = images[i].shape[:2]
-                pn[offsets[k]:offsets[k] + nbytes[k]].reshape(h, w, 3)[...] = images[i]
-            src = self._workspace("frontend_src", total)
-            src[:total].copy_(pinned[:total], non_blocking=True)           # the batch's one H2D
-            hwp = np.array([images[i].shape[:2] + (images[i].shape[1],) for i in idxs], np.int32)
-            fxy = np.array([[p.f, p.f] for p in items], np.float64)
             is_u8 = items[0].dtype == "|u1"
             if is_u8:          # im_scale == 1: resize_im writes the network's uint8 canvas directly
                 u8 = canvas = torch.empty((B, H, W, 3), dtype=torch.uint8, device=self.device)
@@ -711,8 +713,24 @@ class Engine:
                 u8 = self._workspace("frontend_u8", B * Hr * Wr * 3)[:B * Hr * Wr * 3].view(B, Hr, Wr, 3)
                 canvas = torch.empty((B, H, W, 3), dtype=torch.float32, device=self.device)
             resized_hw = np.array([p.resized for p in items], np.int32)
-            N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(src), total, N.ptr(offsets), N.ptr(hwp), N.ptr(fxy), N.ptr(resized_hw),
-                                                       B, 3, N.ptr(u8), Hr, Wr, stream), "ctpn_resize_linear_u8_ragged")
+            fxy = np.array([[p.f, p.f] for p in items], np.float64)
+            if device_images:      # read in place: no staging, no image H2D
+                resize_strided([images[i] for i in idxs], channels, fxy, resized_hw, u8, stream)
+            else:
+                nbytes = [images[i].size for i in idxs]
+                offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
+                total = int(sum(nbytes))
+                pinned = self._pin("frontend_src", (1 << max(20, (total - 1).bit_length()),), torch.uint8)   # grow-only sizes
+                pn = pinned.numpy()
+                for k, i in enumerate(idxs):
+                    h, w = images[i].shape[:2]
+                    pn[offsets[k]:offsets[k] + nbytes[k]].reshape(h, w, 3)[...] = as_bgr(images[i], channels)
+                src = self._workspace("frontend_src", total)
+                src[:total].copy_(pinned[:total], non_blocking=True)           # the batch's one H2D
+                hwp = np.array([images[i].shape[:2] + (images[i].shape[1],) for i in idxs], np.int32)
+                N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(src), total, N.ptr(offsets), N.ptr(hwp), N.ptr(fxy),
+                                                           N.ptr(resized_hw), B, 3, N.ptr(u8), Hr, Wr, stream),
+                        "ctpn_resize_linear_u8_ragged")
             if not is_u8:
                 boffs = np.arange(B, dtype=np.int64) * (Hr * Wr * 3)
                 bhwp = np.concatenate([resized_hw, np.full((B, 1), Wr, np.int32)], axis=1)
@@ -794,14 +812,15 @@ class Engine:
         return out
 
     def detect_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None):
+                            cfg=None, channels="BGR"):
         """ctpn() (demo.py:55-68 minus file I/O) for a list of raw HxWx3 uint8 BGR images of any sizes, all on the device:
         the batches of rois_images (same inputs and batching), then the text-line connector (text_lines) on each batch's
         rois, and one D2H per batch of the packed lines, counts and statuses.  Returns, in input order, (lines float64
         [m,9] (x1,y1,x2,y2,x3,y3,x4,y4,score) in the resize_im frame, f) per image, plus the resize_im output with
         return_resized.  lines is bit-identical to TextDetector(native=True).detect(boxes, scores[:, None], resized.shape[:2])
         on detect_images' output for that image (mode "H" / "O" as cfg.TEST.DETECT_MODE; cfg: the 9 connector constants,
-        None = text_connect_cfg's).  Raises CtpnError where that connector raises (a proposal outside the image width)."""
+        None = text_connect_cfg's).  Raises CtpnError where that connector raises (a proposal outside the image width).
+        images and channels: as for rois_images (host images, or CUDA tensors read in place; BGR or RGB)."""
         if mode not in ("H", "O"):
             raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
         rows = self.result_rows()
@@ -811,18 +830,18 @@ class Engine:
 
         out = [None] * len(images)
         for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
-                                                                "detect_lines_images", after=connect):
+                                                                "detect_lines_images", after=connect, channels=channels):
             per_image = self.split_lines(*self.unpack_lines(out_h.numpy(), len(idxs), rows), im_hw=[p.resized for p in items])
             for k, (i, lines) in enumerate(zip(idxs, per_image)):
                 out[i] = (lines, items[k].f) + ((resized[k],) if return_resized else ())
         return out
 
-    def detect_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200):
+    def detect_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, channels="BGR"):
         """rois_images as test_ctpn returns it: per image (scores float32 [n], boxes float64 [n,4] = rois / im_scale, f), plus
         the resize_im output with return_resized.  Boxes are in the resize_im frame, as TextDetector expects them
-        (draw_boxes divides by f)."""
+        (draw_boxes divides by f).  images and channels: as for rois_images."""
         res = self.rois_images(images, resize=resize, max_batch=max_batch, return_resized=return_resized, scale=scale,
-                               max_scale=max_scale)
+                               max_scale=max_scale, channels=channels)
         return [(r[0][:, 0], r[0][:, 1:5] / np.float64(r[1])) + tuple(r[2:]) for r in res]
 
     # ---- streamed photos: staging, upload and compute overlapped ---------------------------------
@@ -846,7 +865,8 @@ class Engine:
             bufs[(kind, slot)] = buf
         return buf
 
-    def _stream(self, images, split, what, resize, max_batch, return_resized, scale, max_scale, window, compact_rows, after=None):
+    def _stream(self, images, split, what, resize, max_batch, return_resized, scale, max_scale, window, compact_rows, after=None,
+                channels="BGR"):
         """The generator behind stream_rois_images / stream_images / stream_lines_images: run_stream over the batches of
         stream_windows with these stages, on two slots used alternately --
           pack     (worker thread) the batch's rows, row maps, sizes and im_info into the slot's pinned buffer
@@ -857,12 +877,15 @@ class Engine:
                    runs them, into the slot's uint8 canvas; then on the result stream one D2H of the result (and, with
                    return_resized, one of the uint8 canvas);
           finish   waits for that D2H and splits it: split(host buffer, batch) -> one tuple per image.
-        The host blocks only in finish, for the batch it is about to yield."""
+        The host blocks only in finish, for the batch it is about to yield.  A stream of CUDA tensors (its first image
+        decides) packs and uploads the sizes and im_info only, and compute reads the tensors in place
+        (ctpn_resize_linear_u8_strided); each batch holds its tensors until its results have come back."""
         if not 1 <= int(max_batch) <= 64:
             raise ValueError("%s: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)" % what)
         window = 2 * int(max_batch) if window is None else int(window)
         if window < 1:
             raise ValueError("%s: window must be at least 1" % what)
+        check_channels(channels, what)
         if getattr(self, "_copy_stream", None) is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
             self._result_stream = torch.cuda.Stream(device=self.device)
@@ -871,19 +894,29 @@ class Engine:
         lut = self._mean_lut()
         copied, computed, returned = [None, None], [None, None], [None, None]     # per slot: events of its last H2D / compute / D2H
 
+        device_images = []                      # [whether the stream's images are CUDA tensors], set by its first image
+
         def prepare(im, index):
-            a = im.numpy() if torch.is_tensor(im) else np.asarray(im)
+            dev = on_device(im, self.device, what, index)
+            if not device_images:
+                device_images.append(dev)
+            elif dev != device_images[0]:
+                raise ValueError("%s: image %d is %s but the stream's first image is %s; one stream takes host images or CUDA "
+                                 "tensors, not both" % ((what, index) + (("a CUDA tensor", "a host image") if dev else
+                                                                         ("a host image", "a CUDA tensor"))))
+            a = im if dev else (im.numpy() if torch.is_tensor(im) else np.asarray(im))
             return a, frontend_plan([a], resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg, first=index)[0]
 
         def pack_on_host(batch, slot):          # calling thread: sizes only, and the pinned buffer (grow-only)
-            lay = stream_layout(batch.items, [im.shape[:2] for im in batch.images], compact_rows)
+            lay = stream_layout(batch.items, [tuple(im.shape[:2]) for im in batch.images], compact_rows,
+                                sources=not device_images[0])
             return lay, self._stream_buffer("pin_src", slot, lay.total), copied[slot]
 
         def pack(batch, slot, staged):          # worker thread: row copies (numpy releases the GIL for them)
             lay, pinned, free = staged
             if free is not None:
                 free.synchronize()
-            stream_pack(pinned.numpy(), lay, batch)
+            stream_pack(pinned.numpy(), lay, batch, channels)
             return lay, pinned
 
         def upload(batch, slot, packed):
@@ -908,14 +941,17 @@ class Engine:
             is_u8 = items[0].dtype == "|u1"
             Hr, Wr = (H, W) if is_u8 else (max(p.resized[0] for p in items), max(p.resized[1] for p in items))
             u8 = self._stream_buffer("u8", slot, B * Hr * Wr * 3)[:B * Hr * Wr * 3].view(B, Hr, Wr, 3)
-            hwp = np.array([im.shape[:2] + (im.shape[1],) for im in batch.images], np.int32)
             fxy = np.array([[p.f, p.f] for p in items], np.float64)
             resized_hw = np.array([p.resized for p in items], np.int32)
-            if lay.maps is None:
+            if lay.offsets is None:
+                resize_strided(batch.images, channels, fxy, resized_hw, u8, stream)
+            elif lay.maps is None:
+                hwp = np.array([im.shape[:2] + (im.shape[1],) for im in batch.images], np.int32)
                 N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(dev), lay.map_base, N.ptr(lay.offsets), N.ptr(hwp), N.ptr(fxy),
                                                            N.ptr(resized_hw), B, 3, N.ptr(u8), Hr, Wr, stream),
                         "ctpn_resize_linear_u8_ragged")
             else:
+                hwp = np.array([im.shape[:2] + (im.shape[1],) for im in batch.images], np.int32)
                 maps = dev[lay.map_base:lay.sizes_at].view(torch.int32)
                 N.check(N.lib.ctpn_resize_linear_u8_ragged_rows(N.ptr(dev), lay.map_base, N.ptr(lay.offsets), N.ptr(hwp),
                                                                 N.ptr(lay.stored), N.ptr(maps), maps.numel(), N.ptr(lay.maps),
@@ -949,7 +985,8 @@ class Engine:
                     res_h.copy_(u8, non_blocking=True)
                 returned[slot] = torch.cuda.Event()
                 returned[slot].record(result_stream)
-            return out_h, res_h, returned[slot], (packed, result)       # the device results live until the D2H has run
+            # the device results and the batch's input tensors live until the D2H, which follows the compute, has run
+            return out_h, res_h, returned[slot], (packed, result, batch.images)
 
         def finish(batch, handle):
             out_h, res_h, ev, _keep = handle
@@ -975,7 +1012,7 @@ class Engine:
         return stream()
 
     def stream_rois_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, window=None,
-                           compact_rows=True):
+                           compact_rows=True, channels="BGR"):
         """rois_images for any iterable of raw HxWx3 uint8 BGR images (e.g. a generator that decodes files), as a generator:
         yields, in input order, the tuple rois_images returns for each image -- bit-identical to it -- while later images
         are still being pulled, packed, uploaded and computed (see _stream for the stages that overlap).  window: how
@@ -984,17 +1021,25 @@ class Engine:
         photo is uploaded as the rows resize_im reads only (FrontendStep.rows; compact_rows=False uploads every image
         whole).  A bad image raises frontend_plan's ValueError when the stream reaches it, after the results of all images
         before it.  Closing the generator early waits for the work in flight and leaves the engine ready for any other
-        call; one stream per engine can be open at a time."""
+        call; one stream per engine can be open at a time.
+
+        The images may instead all be CUDA uint8 [H, W, 3] tensors on this engine's device, at any strides, as rois_images
+        takes them: then only the sizes and im_info are uploaded, and the kernels read the tensors in place.  They must be
+        ready on the stream that was current when the generator was created (torch's rule); the engine synchronises
+        nothing for them.  The stream keeps each batch's tensors referenced until that batch's results have come back, so
+        a caller may drop its own references as soon as the generator has pulled them; the window then also bounds the
+        device memory the stream holds.  An image of the other kind than the stream's first (host or device) raises
+        ValueError when the stream reaches it, like a bad image.  channels: as for rois_images."""
         rows = self.result_rows()
 
         def split(out_h, batch):
             return [(r, p.im_scale, p.f) for r, p in zip(self._split_results(out_h, len(batch.items), rows), batch.items)]
 
         return self._stream(images, split, "stream_rois_images", resize, max_batch, return_resized, scale, max_scale, window,
-                            compact_rows)
+                            compact_rows, channels=channels)
 
     def stream_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, window=None,
-                      compact_rows=True):
+                      compact_rows=True, channels="BGR"):
         """detect_images as a generator over any iterable of raw photos: see stream_rois_images."""
         rows = self.result_rows()
 
@@ -1003,10 +1048,10 @@ class Engine:
                     for r, p in zip(self._split_results(out_h, len(batch.items), rows), batch.items)]
 
         return self._stream(images, split, "stream_images", resize, max_batch, return_resized, scale, max_scale, window,
-                            compact_rows)
+                            compact_rows, channels=channels)
 
     def stream_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None, window=None, compact_rows=True):
+                            cfg=None, window=None, compact_rows=True, channels="BGR"):
         """detect_lines_images as a generator over any iterable of raw photos: see stream_rois_images; the connector runs
         on each batch's rois on the device and only the lines come back.  Raises CtpnError where detect_lines_images does."""
         if mode not in ("H", "O"):
@@ -1019,7 +1064,7 @@ class Engine:
             return [(ln, p.f) for ln, p in zip(lines, batch.items)]
 
         return self._stream(images, split, "stream_lines_images", resize, max_batch, return_resized, scale, max_scale, window,
-                            compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg))
+                            compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg), channels=channels)
 
     def _connect(self, packed, items, mode, cfg):
         """The text-line connector on one batch's packed rois -> the packed lines (unpack_lines), on the device."""
@@ -1128,6 +1173,75 @@ def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None, firs
     return out
 
 
+# ---- photos already in device memory ------------------------------------------------------------------------------------
+CHANNELS = ("BGR", "RGB")
+
+
+def check_channels(channels, what):
+    if channels not in CHANNELS:
+        raise ValueError("%s: channels must be 'BGR' or 'RGB' (got %r)" % (what, channels))
+
+
+def as_bgr(a, channels):
+    """A host image as the BGR view the packing copy reads (no copy of its own)."""
+    return a[:, :, ::-1] if channels == "RGB" else a
+
+
+def on_device(im, device, what, index):
+    """Whether image `index` of a raw-photo call is a CUDA tensor, which must then be on the engine's `device` (its dtype and
+    shape are frontend_plan's to check).  Anything else is a host image, CPU tensors included."""
+    if not (torch.is_tensor(im) and im.is_cuda):
+        return False
+    if im.device != device:
+        raise ValueError("%s: image %d is on %s, the engine runs on %s" % (what, index, im.device, device))
+    return True
+
+
+def images_on_device(images, device, what):
+    """True when every image of a list call is a CUDA tensor, False when none is; a mixed list raises ValueError."""
+    kinds = [on_device(im, device, what, i) for i, im in enumerate(images)]
+    if any(kinds) and not all(kinds):
+        i = kinds.index(not kinds[0])
+        raise ValueError("%s: image %d is %s but image 0 is %s; one call takes host images or CUDA tensors, not both"
+                         % (what, i, *(("a CUDA tensor", "a host image") if kinds[i] else ("a host image", "a CUDA tensor"))))
+    return bool(kinds) and kinds[0]
+
+
+def strided_descriptor(address, nbytes, offset, strides, channels="BGR"):
+    """ctpn_resize_linear_u8_strided's descriptor of an HxWx3 uint8 image in the allocation at device `address` of `nbytes`
+    bytes, whose sample (0, 0, 0) lies at byte `offset` and whose byte strides are strides = (row, column, channel) ->
+    (address, nbytes, offset, (row, column, channel)) reading it as BGR.  channels="RGB": the image holds RGB, so the kernel
+    starts at channel 2 and steps backwards."""
+    check_channels(channels, "strided_descriptor")
+    rs, cs, ks = (int(s) for s in strides)
+    offset = int(offset)
+    if channels == "RGB":
+        offset, ks = offset + 2 * ks, -ks
+    return int(address), int(nbytes), offset, (rs, cs, ks)
+
+
+def tensor_descriptor(t, channels="BGR"):
+    """strided_descriptor of a uint8 [H, W, 3] tensor: its storage is the allocation (uint8, so elements are bytes)."""
+    st = t.untyped_storage()
+    return strided_descriptor(st.data_ptr(), st.nbytes(), t.storage_offset(), t.stride(), channels)
+
+
+def resize_strided(tensors, channels, fxy, dst_hw, dst, stream):
+    """resize_im of CUDA uint8 [h, w, 3] tensors read in place into the uint8 canvas dst [B, H, W, 3]
+    (ctpn_resize_linear_u8_strided)."""
+    B = len(tensors)
+    desc = [tensor_descriptor(t, channels) for t in tensors]
+    addr = np.array([d[0] for d in desc], np.uint64)
+    nbytes = np.array([d[1] for d in desc], np.uint64)
+    offs = np.array([d[2] for d in desc], np.int64)
+    strides = np.array([d[3] for d in desc], np.int64)
+    hw = np.array([tuple(t.shape[:2]) for t in tensors], np.int32)
+    N.check(N.lib.ctpn_resize_linear_u8_strided(N.ptr(addr), N.ptr(nbytes), N.ptr(offs), N.ptr(strides), N.ptr(hw),
+                                                N.ptr(np.ascontiguousarray(fxy, np.float64)),
+                                                N.ptr(np.ascontiguousarray(dst_hw, np.int32)), B, N.ptr(dst),
+                                                int(dst.shape[1]), int(dst.shape[2]), stream), "ctpn_resize_linear_u8_strided")
+
+
 # ---- streamed photos: the parts of Engine._stream that need no device ---------------------------------------------------
 StreamBatch = collections.namedtuple("StreamBatch", "idxs items images canvas")
 # One batch's upload: [the images' rows, back to back][row maps, int32][blob sizes, int32 B x 2][feature sizes, int32 B x 2]
@@ -1137,10 +1251,13 @@ StreamBatch = collections.namedtuple("StreamBatch", "idxs items images canvas")
 StreamLayout = collections.namedtuple("StreamLayout", "offsets stored rows map_base maps sizes_at total")
 
 
-def stream_layout(items, shapes, compact_rows=True):
+def stream_layout(items, shapes, compact_rows=True, sources=True):
     """Where everything of one batch goes in its upload buffer: items are the batch's FrontendSteps, shapes its images'
     (h, w).  An image is sent as its FrontendStep.rows when it has them (and compact_rows), else whole; if any image of the
-    batch is compacted, every image gets a row map (the identity for a whole one)."""
+    batch is compacted, every image gets a row map (the identity for a whole one).  sources=False (images the device reads
+    in place): the buffer holds the sizes and im_info only."""
+    if not sources:
+        return StreamLayout(None, None, None, 0, None, 0, 28 * len(items))
     rows = [p.rows if compact_rows else None for p in items]
     stored = np.array([h if r is None else len(r) for (h, w), r in zip(shapes, rows)], np.int32)
     nbytes = [int(n) * int(w) * 3 for n, (h, w) in zip(stored, shapes)]
@@ -1154,13 +1271,14 @@ def stream_layout(items, shapes, compact_rows=True):
     return StreamLayout(offsets, stored, rows, map_base, maps, sizes_at, sizes_at + 28 * len(items))
 
 
-def stream_pack(buf, lay, batch):
-    """Fills a batch's upload buffer (uint8 ndarray of at least lay.total bytes) as stream_layout laid it out."""
+def stream_pack(buf, lay, batch, channels="BGR"):
+    """Fills a batch's upload buffer (uint8 ndarray of at least lay.total bytes) as stream_layout laid it out; RGB images
+    (channels="RGB") are flipped to BGR by the row copies."""
     B = len(batch.items)
-    for k, im in enumerate(batch.images):
+    for k, im in enumerate(batch.images if lay.offsets is not None else ()):
         h, w = im.shape[:2]
         n, r = int(lay.stored[k]), lay.rows[k]
-        dst = buf[lay.offsets[k]:lay.offsets[k] + n * w * 3].reshape(n, w, 3)
+        dst = as_bgr(buf[lay.offsets[k]:lay.offsets[k] + n * w * 3].reshape(n, w, 3), channels)
         if r is None:
             dst[...] = im
         else:
