@@ -24,6 +24,7 @@
  *   ctpn_resize_linear_u8_ragged / ctpn_image_blob_f32_ragged   the same two, for a batch of images of different sizes
  *   ctpn_resize_linear_u8_ragged_rows     the ragged resize on sources that hold only the rows it reads
  *   ctpn_resize_linear_u8_strided         the ragged resize on images read in place at any byte strides
+ *   ctpn_resize_linear_u8_yuv420          the same on YUV 4:2:0 frames, with cv2.cvtColor's conversion to BGR
  *   ctpn_text_filter_nms_host / ctpn_text_groups_host / ctpn_text_lines_host / ctpn_text_lines (batched, device)
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
@@ -272,6 +273,23 @@ int ctpn_resize_linear_u8_ragged_rows(const void *src, size_t src_elems, const l
 int ctpn_resize_linear_u8_strided(const void *const *src, const size_t *src_bytes, const long long *src_offset,
                                   const long long *src_strides, const int *src_hw, const double *fxy, const int *dst_hw, int B,
                                   void *dst, int H, int W, void *stream);
+
+/* ctpn_resize_linear_u8_strided for YUV 4:2:0 frames read in place (e.g. NV12 surfaces of a video decoder): image b is
+ * the (h, w) = src_hw[2b..2b+1] frame whose planes p = 0, 1, 2 (Y, U, V) have their sample (y, x) at byte
+ *   planes[3b + p] + plane_offset[3b + p] + y * plane_strides[6b + 2p] + x * plane_strides[6b + 2p + 1]
+ * of the allocation planes[3b + p] (a DEVICE address) of plane_bytes[3b + p] bytes; Y is h x w, U and V are h/2 x w/2.
+ * Strides are signed and may be zero, so NV12 / NV21 (interleaved chroma: column stride 2, U and V one byte apart), I420 /
+ * YV12, pitched surfaces, planes in separate allocations and even-offset crops are all descriptors.  Each sample is
+ * converted to BGR as cv2.cvtColor(COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) converts it (BT.601 limited range, 20-bit
+ * fixed point, nearest chroma), then resized as ctpn_resize_linear_u8_strided resizes; the output, written exactly as that
+ * call writes it, is bit-identical to it on the cvtColor output.  planes, plane_bytes, plane_offset, plane_strides,
+ * src_hw, fxy and dst_hw are HOST arrays (1 <= B <= 64).  Validated before any CUDA call, with the size, scale, dst_hw and
+ * canvas rules of ctpn_resize_linear_u8_ragged and in addition (CTPN_ERR_INVALID naming the image and the plane): h and w
+ * even; a NULL plane; the lowest and the highest byte each plane's box can touch must lie in [0, plane_bytes); column
+ * strides must fit in 32 bits. */
+int ctpn_resize_linear_u8_yuv420(const void *const *planes, const size_t *plane_bytes, const long long *plane_offset,
+                                 const long long *plane_strides, const int *src_hw, const double *fxy, const int *dst_hw,
+                                 int B, void *dst, int H, int W, void *stream);
 
 /* CRC-32C (Castagnoli) of a host buffer, continuing from `crc` (0 to start): the per-tensor checksum of TF checkpoint V2
  * files, used by the weight importer (ctpn_b200/tf_import.py) to verify every tensor it loads. */

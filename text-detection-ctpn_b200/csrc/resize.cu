@@ -20,7 +20,8 @@
 // The *_ragged entry points run both for a batch of images of different sizes (Engine.rois_images); they share the
 // per-pixel functions below with the single-image kernels.  ctpn_resize_linear_u8_ragged_rows is the ragged resize on
 // sources that hold only the rows it reads (Engine.stream_rois_images uploads camera photos that way), and
-// ctpn_resize_linear_u8_strided the ragged resize on images read in place at any byte strides (CUDA tensors of callers).
+// ctpn_resize_linear_u8_strided the ragged resize on images read in place at any byte strides (CUDA tensors of callers);
+// ctpn_resize_linear_u8_yuv420 converts YUV 4:2:0 frames read in place to BGR as cv2.cvtColor does, inside that resize.
 #include "common.cuh"
 
 namespace ctpn {
@@ -71,11 +72,34 @@ struct StridedPixels {
     return __ldg(r + ((long long)x * col_stride + (long long)c * chan_stride));
   }
 };
+// ... or converted from YUV 4:2:0 planes on the fly (ctpn_resize_linear_u8_yuv420: video frames read in place), exactly as
+// cv2.cvtColor(COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) converts them: BT.601 limited range in 20-bit fixed point,
+// nearest chroma -- chroma sample (y >> 1, x >> 1) serves luma sample (y, x).  Every term fits in int32 and >> is
+// arithmetic, as in OpenCV's 4:2:0 converters (restated and pinned against cv2 in oracle/yuv.py).  The row handle is a
+// luma row plus the chroma rows of row >> 1; rows and columns come in clamped, so the chroma indices are in range too.
+struct Yuv420Pixels {
+  const uint8_t *y, *u, *v;    // sample (0, 0) of each plane
+  long long y_row, u_row, v_row;
+  int y_col, u_col, v_col;
+  struct Row {
+    const uint8_t *y, *u, *v;
+  };
+  __device__ __forceinline__ Row row(int r) const {
+    return Row{y + (long long)r * y_row, u + (long long)(r >> 1) * u_row, v + (long long)(r >> 1) * v_row};
+  }
+  __device__ __forceinline__ uint8_t at(const Row &r, int x, int c) const {
+    const int Y = __ldg(r.y + (long long)x * y_col);
+    const int U = __ldg(r.u + (long long)(x >> 1) * u_col) - 128, V = __ldg(r.v + (long long)(x >> 1) * v_col) - 128;
+    const int yy = max(Y - 16, 0) * 1220542 + (1 << 19);
+    const int t = c == 0 ? yy + 2116026 * U : c == 1 ? yy - 852492 * V - 409993 * U : yy + 1673527 * V;
+    return (uint8_t)min(max(t >> 20, 0), 255);
+  }
+};
 
 // One output pixel of cv2.resize(INTER_LINEAR) of a uint8 image of sh x sw pixels and C channels -> o[C].  Shared by
 // every uint8 resize kernel: a ragged or strided batch is bit-identical to single-image runs by construction.  Taps,
-// weights, the INTER_AREA route and rounding come from the source geometry (sh, sw); only the address of a sample goes
-// through the accessor `src`.
+// weights, the INTER_AREA route and rounding come from the source geometry (sh, sw); only the value of a sample comes from
+// the accessor `src`, whose row handle is whatever its row() returns.
 template <class Src>
 __device__ __forceinline__ void resize_u8_pixel(const Src src, int sh, int sw, int C, int dx, int dy, double scale_x,
                                                 double scale_y, bool area2, uint8_t *__restrict__ o) {
@@ -85,7 +109,7 @@ __device__ __forceinline__ void resize_u8_pixel(const Src src, int sh, int sw, i
     for (int c = 0; c < C; ++c) {
       int sum = 0;
       for (int yy = 0; yy < ny; ++yy) {
-        const uint8_t *r = src.row(y0 + yy);
+        const auto r = src.row(y0 + yy);
         for (int xx = 0; xx < nx; ++xx) sum += src.at(r, x0 + xx, c);
       }
       int v = (ny * nx == 4) ? (sum + 2) >> 2 : __float2int_rn(__fdiv_rn((float)sum, (float)(ny * nx)));
@@ -96,7 +120,7 @@ __device__ __forceinline__ void resize_u8_pixel(const Src src, int sh, int sw, i
   int sx0, sx1, a0, a1, sy0, sy1, b0, b1;
   resize_taps(dx, sw, scale_x, true, sx0, sx1, a0, a1);
   resize_taps(dy, sh, scale_y, false, sy0, sy1, b0, b1);
-  const uint8_t *r0 = src.row(sy0), *r1 = src.row(sy1);
+  const auto r0 = src.row(sy0), r1 = src.row(sy1);
   for (int c = 0; c < C; ++c) {
     const int h0 = src.at(r0, sx0, c) * a0 + src.at(r0, sx1, c) * a1;
     const int h1 = src.at(r1, sx0, c) * a0 + src.at(r1, sx1, c) * a1;
@@ -244,6 +268,36 @@ __global__ void __launch_bounds__(256) resize_linear_u8_strided_kernel(uint8_t *
                                                                        const __grid_constant__ StridedResize p) {
   const int b = blockIdx.y, dh = p.dh[b], dw = p.dw[b];
   const StridedPixels src_b{p.base[b], p.row_stride[b], p.col_stride[b], p.chan_stride[b]};
+  uint8_t *out = dst + (size_t)b * p.H * p.W * 3;
+  const long long total = (long long)dh * dw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int dx = (int)(i % dw), dy = (int)(i / dw);
+    resize_u8_pixel(src_b, p.sh[b], p.sw[b], 3, dx, dy, p.scale_x[b], p.scale_y[b], (p.area2 >> b) & 1,
+                    out + ((size_t)dy * p.W + dx) * 3);
+  }
+}
+
+// YUV 4:2:0 frames read in place (ctpn_resize_linear_u8_yuv420), written as the strided kernel writes them.  Three planes
+// per image take 92 bytes of descriptors, so 64 images (5.9 KB) would exceed the 4 KB of kernel parameters; the host
+// launches chunks of up to kYuvChunk images, each writing its own canvas slices.
+constexpr int kYuvChunk = 32;
+struct Yuv420Resize {
+  const uint8_t *plane[kYuvChunk][3];  // sample (0, 0) of the Y, U and V plane of image b
+  long long row_stride[kYuvChunk][3];
+  int col_stride[kYuvChunk][3];
+  double scale_x[kYuvChunk], scale_y[kYuvChunk];
+  int sh[kYuvChunk], sw[kYuvChunk], dh[kYuvChunk], dw[kYuvChunk];
+  unsigned area2;                      // bit b: exact 1/2 in both directions
+  int H, W;
+};
+static_assert(sizeof(Yuv420Resize) + sizeof(void *) <= 4096, "yuv420 resize parameters exceed 4 KB");
+
+__global__ void __launch_bounds__(256) resize_linear_u8_yuv420_kernel(uint8_t *__restrict__ dst,
+                                                                      const __grid_constant__ Yuv420Resize p) {
+  const int b = blockIdx.y, dh = p.dh[b], dw = p.dw[b];
+  const Yuv420Pixels src_b{p.plane[b][0], p.plane[b][1], p.plane[b][2],
+                           p.row_stride[b][0], p.row_stride[b][1], p.row_stride[b][2],
+                           p.col_stride[b][0], p.col_stride[b][1], p.col_stride[b][2]};
   uint8_t *out = dst + (size_t)b * p.H * p.W * 3;
   const long long total = (long long)dh * dw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -511,5 +565,73 @@ extern "C" int ctpn_resize_linear_u8_strided(const void *const *src, const size_
   ProfScope prof("resize_linear_u8_strided", (double)work, (cudaStream_t)stream);
   resize_linear_u8_strided_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint8_t *)dst, p);
   CTPN_LAUNCH_CHECK();
+  return CTPN_OK;
+}
+
+extern "C" int ctpn_resize_linear_u8_yuv420(const void *const *planes, const size_t *plane_bytes, const long long *plane_offset,
+                                            const long long *plane_strides, const int *src_hw, const double *fxy,
+                                            const int *dst_hw, int B, void *dst, int H, int W, void *stream) {
+  const char *fn = "ctpn_resize_linear_u8_yuv420";
+  static const char *const kPlane[3] = {"Y", "U", "V"};
+  CTPN_REQUIRE(dst, "%s: null pointer", fn);
+  CTPN_REQUIRE(planes && plane_bytes && plane_offset && plane_strides && src_hw && fxy && dst_hw, "%s: null descriptor array",
+               fn);
+  CTPN_REQUIRE(B >= 1 && B <= kRaggedMax, "%s: B = %d, must be 1..%d", fn, B, kRaggedMax);
+  CTPN_REQUIRE(H > 0 && W > 0, "%s: bad canvas %d x %d", fn, H, W);
+  Yuv420Resize chunk[(kRaggedMax + kYuvChunk - 1) / kYuvChunk];
+  memset(chunk, 0, sizeof(chunk));
+  long long max_pixels[(kRaggedMax + kYuvChunk - 1) / kYuvChunk] = {}, work = 0;
+  for (int b = 0; b < B; ++b) {
+    const int sh = src_hw[2 * b], sw = src_hw[2 * b + 1];
+    CTPN_REQUIRE(sh > 0 && sw > 0 && sh % 2 == 0 && sw % 2 == 0, "%s: image %d: source size %d x %d must be even and positive",
+                 fn, b, sh, sw);
+    Yuv420Resize &p = chunk[b / kYuvChunk];
+    const int k = b % kYuvChunk;
+    for (int q = 0; q < 3; ++q) {
+      const int i = 3 * b + q;
+      const long long off = plane_offset[i], *st = plane_strides + 2 * i;
+      CTPN_REQUIRE(planes[i], "%s: image %d: null %s plane", fn, b, kPlane[q]);
+      CTPN_REQUIRE(st[1] >= INT_MIN && st[1] <= INT_MAX, "%s: image %d: %s plane column stride %lld outside the 32-bit range",
+                   fn, b, kPlane[q], st[1]);
+      // lowest and highest byte of the plane's box (h x w luma, h/2 x w/2 chroma); 128-bit, so no stride can wrap them
+      __int128 lo = off, hi = off;
+      const long long extent[2] = {(q ? sh / 2 : sh) - 1, (q ? sw / 2 : sw) - 1};
+      for (int d = 0; d < 2; ++d) {
+        const __int128 span = (__int128)extent[d] * st[d];
+        (span < 0 ? lo : hi) += span;
+      }
+      CTPN_REQUIRE(lo >= 0 && hi < (__int128)plane_bytes[i],
+                   "%s: image %d: the %s plane spans bytes [%lld, %lld] of its allocation, outside [0, %zu)", fn, b, kPlane[q],
+                   (long long)std::max<__int128>(std::min<__int128>(lo, LLONG_MAX), LLONG_MIN),
+                   (long long)std::max<__int128>(std::min<__int128>(hi, LLONG_MAX), LLONG_MIN), plane_bytes[i]);
+      p.plane[k][q] = (const uint8_t *)planes[i] + off;
+      p.row_stride[k][q] = st[0];
+      p.col_stride[k][q] = (int)st[1];
+    }
+    int eh = 0, ew = 0;
+    const int rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew);
+    if (rc) return rc;
+    p.H = H;
+    p.W = W;
+    p.sh[k] = sh;
+    p.sw[k] = sw;
+    p.dh[k] = eh;
+    p.dw[k] = ew;
+    p.scale_x[k] = 1.0 / fxy[2 * b];
+    p.scale_y[k] = 1.0 / fxy[2 * b + 1];
+    if (p.scale_x[k] == 2.0 && p.scale_y[k] == 2.0) p.area2 |= 1u << k;
+    max_pixels[b / kYuvChunk] = std::max(max_pixels[b / kYuvChunk], (long long)eh * ew);
+    work += (long long)eh * ew * 3;
+  }
+  ProfScope prof("resize_linear_u8_yuv420", (double)work, (cudaStream_t)stream);
+  for (int first = 0; first < B; first += kYuvChunk) {
+    const int nb = std::min(kYuvChunk, B - first);
+    dim3 grid;
+    int rc = ragged_grid(nb, max_pixels[first / kYuvChunk], &grid);
+    if (rc) return rc;
+    resize_linear_u8_yuv420_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((uint8_t *)dst + (size_t)first * H * W * 3,
+                                                                            chunk[first / kYuvChunk]);
+    CTPN_LAUNCH_CHECK();
+  }
   return CTPN_OK;
 }

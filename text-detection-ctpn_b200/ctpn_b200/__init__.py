@@ -2,7 +2,7 @@
 eragonruan/text-detection-ctpn).  Importing the package loads libctpn_b200.so; there is no
 CPU fallback."""
 from ._native import CtpnError, LIB_PATH, lib  # noqa: F401
-from .engine import Engine, frontend_plan, load_weight_file, ragged_plan  # noqa: F401
+from .engine import YUV420, Engine, frontend_plan, load_weight_file, ragged_plan  # noqa: F401
 from .session import Session  # noqa: F401
 
-__all__ = ["Engine", "Session", "CtpnError", "load_weight_file", "ragged_plan", "frontend_plan", "LIB_PATH"]
+__all__ = ["Engine", "Session", "CtpnError", "YUV420", "load_weight_file", "ragged_plan", "frontend_plan", "LIB_PATH"]

@@ -59,6 +59,7 @@ SIGNATURES = {
     "ctpn_image_blob_f32_ragged": (_i, [_p, _z, _p, _p, _p, _p, _p, _i, _p, _i, _i, _p]),
     "ctpn_resize_linear_u8_ragged_rows": (_i, [_p, _z, _p, _p, _p, _p, _z, _p, _p, _p, _i, _i, _p, _i, _i, _p]),
     "ctpn_resize_linear_u8_strided": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _p]),
+    "ctpn_resize_linear_u8_yuv420": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _p, _i, _i, _p]),
     "ctpn_nms_workspace_bytes": (_z, [_i, _i]),
     "ctpn_nms_sorted": (_i, [_p, _p, _i, _i, _f, _i, _p, _p, _p, _z, _p]),
     "ctpn_proposals_workspace_bytes": (_z, [_i, _i, _i, _i]),

@@ -675,7 +675,13 @@ class Engine:
         when the call is made (torch's rule); the engine synchronises nothing for them.  A list that mixes host images and
         CUDA tensors, or a tensor on another device, raises ValueError before any device work.  channels="RGB": every image
         of the call holds RGB (as torchvision decodes it) -- host images are flipped inside the packing copy, tensors are
-        read through a negative channel stride."""
+        read through a negative channel stride.
+
+        Or the images may all be YUV420 frames (video frames: NV12, NV21, I420, YV12 planes) on this engine's device:
+        ctpn_resize_linear_u8_yuv420 reads the planes in place and converts each sample as cv2.cvtColor does, so the results
+        equal those of the same call on cv2.cvtColor(frame, COLOR_YUV2BGR_*) -- return_resized included.  The stream rule
+        above applies to the planes; a frame with odd sides, a plane on another device or channels="RGB" raises ValueError
+        before any device work."""
         out = [None] * len(images)
         rows = self.result_rows()
         for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
@@ -695,7 +701,7 @@ class Engine:
             raise ValueError("%s: max_batch must be 1..64 (the ragged front-end kernels take up to 64 images)" % what)
         check_channels(channels, what)
         images = list(images)
-        device_images = images_on_device(images, self.device, what)
+        device_images = images_on_device(images, self.device, what, channels)
         if not device_images:
             images = [im.numpy() if torch.is_tensor(im) else np.asarray(im) for im in images]
         plan = frontend_plan(images, resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg)
@@ -715,7 +721,7 @@ class Engine:
             resized_hw = np.array([p.resized for p in items], np.int32)
             fxy = np.array([[p.f, p.f] for p in items], np.float64)
             if device_images:      # read in place: no staging, no image H2D
-                resize_strided([images[i] for i in idxs], channels, fxy, resized_hw, u8, stream)
+                resize_in_place([images[i] for i in idxs], device_images, channels, fxy, resized_hw, u8, stream)
             else:
                 nbytes = [images[i].size for i in idxs]
                 offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
@@ -894,16 +900,14 @@ class Engine:
         lut = self._mean_lut()
         copied, computed, returned = [None, None], [None, None], [None, None]     # per slot: events of its last H2D / compute / D2H
 
-        device_images = []                      # [whether the stream's images are CUDA tensors], set by its first image
+        device_images = []                      # [the kind (on_device) of the stream's images], set by its first image
 
         def prepare(im, index):
-            dev = on_device(im, self.device, what, index)
+            dev = on_device(im, self.device, what, index, channels)
             if not device_images:
                 device_images.append(dev)
             elif dev != device_images[0]:
-                raise ValueError("%s: image %d is %s but the stream's first image is %s; one stream takes host images or CUDA "
-                                 "tensors, not both" % ((what, index) + (("a CUDA tensor", "a host image") if dev else
-                                                                         ("a host image", "a CUDA tensor"))))
+                raise mixed_kinds(what, index, dev, device_images[0], "the stream's first image")
             a = im if dev else (im.numpy() if torch.is_tensor(im) else np.asarray(im))
             return a, frontend_plan([a], resize=resize, scale=scale, max_scale=max_scale, cfg=self.cfg, first=index)[0]
 
@@ -944,7 +948,7 @@ class Engine:
             fxy = np.array([[p.f, p.f] for p in items], np.float64)
             resized_hw = np.array([p.resized for p in items], np.int32)
             if lay.offsets is None:
-                resize_strided(batch.images, channels, fxy, resized_hw, u8, stream)
+                resize_in_place(batch.images, device_images[0], channels, fxy, resized_hw, u8, stream)
             elif lay.maps is None:
                 hwp = np.array([im.shape[:2] + (im.shape[1],) for im in batch.images], np.int32)
                 N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(dev), lay.map_base, N.ptr(lay.offsets), N.ptr(hwp), N.ptr(fxy),
@@ -1028,8 +1032,9 @@ class Engine:
         ready on the stream that was current when the generator was created (torch's rule); the engine synchronises
         nothing for them.  The stream keeps each batch's tensors referenced until that batch's results have come back, so
         a caller may drop its own references as soon as the generator has pulled them; the window then also bounds the
-        device memory the stream holds.  An image of the other kind than the stream's first (host or device) raises
-        ValueError when the stream reaches it, like a bad image.  channels: as for rois_images."""
+        device memory the stream holds.  YUV420 frames stream the same way (see rois_images), their planes held as tensors
+        are.  An image of another kind than the stream's first (host image, CUDA tensor or YUV420 frame) raises ValueError
+        when the stream reaches it, like a bad image.  channels: as for rois_images."""
         rows = self.result_rows()
 
         def split(out_h, batch):
@@ -1133,14 +1138,17 @@ def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None, firs
       dtype     '|u1' when im_scale == 1 (the uint8 image is the blob), else '<f4' (the float32 rescale),
       rows      the source rows resize_im reads (frontend_rows, as a tuple) when they are at most 3/4 of the image -- a
                 streamed upload then sends only those (Engine.stream_rois_images) -- or None: send the image densely.
-    Error messages number the images from `first` (a stream plans its images one at a time).  Raises ValueError when an image is not HxWx3 uint8, a resize would be empty or a blob side would be under 16."""
+    Error messages number the images from `first` (a stream plans its images one at a time).  Raises ValueError when an image is not HxWx3 uint8, a resize would be empty or a blob side would be under 16.
+    A YUV420 frame plans as the BGR image it converts to; one with odd sides or malformed planes raises ValueError."""
     c = dict(DEFAULT_CFG)
     if cfg:
         c.update(cfg)
     target, max_size = float(c["SCALES"][0]), float(c["MAX_SIZE"])
     out = []
     for i, s in enumerate(shapes, int(first)):
-        if hasattr(s, "shape") and hasattr(s, "dtype"):
+        if isinstance(s, YUV420):
+            s = s.hw("frontend_plan", i)
+        elif hasattr(s, "shape") and hasattr(s, "dtype"):
             if len(s.shape) != 3 or s.shape[2] != 3 or str(s.dtype) not in ("uint8", "torch.uint8"):
                 raise ValueError("frontend_plan: image %d must be HxWx3 uint8 (got %s %s)" % (i, tuple(s.shape), s.dtype))
             s = tuple(s.shape)
@@ -1187,24 +1195,115 @@ def as_bgr(a, channels):
     return a[:, :, ::-1] if channels == "RGB" else a
 
 
-def on_device(im, device, what, index):
-    """Whether image `index` of a raw-photo call is a CUDA tensor, which must then be on the engine's `device` (its dtype and
-    shape are frontend_plan's to check).  Anything else is a host image, CPU tensors included."""
+class YUV420(collections.namedtuple("YUV420", "y u v")):
+    """A YUV 4:2:0 video frame in device memory, as the raw-photo calls of Engine take it: y a uint8 [H, W] tensor, u and
+    v uint8 [H/2, W/2] tensors, H and W even, at any strides (views into one buffer, or separate allocations).  The calls
+    convert it to BGR as cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) does -- BT.601 limited range,
+    nearest chroma -- inside the resize (ctpn_resize_linear_u8_yuv420), and return what they return on that BGR image.
+    That is cv2.cvtColor's conversion, not the one behind cv2.VideoCapture's BGR frames (FFmpeg's swscale rounds
+    differently).  shape is that of the BGR image, (H, W, 3)."""
+    __slots__ = ()
+    LAYOUTS = ("NV12", "NV21", "I420", "YV12")
+
+    @property
+    def shape(self):
+        return tuple(int(s) for s in self.y.shape[:2]) + (3,)
+
+    @classmethod
+    def from_buffer(cls, t, layout):
+        """Views of the planes of one uint8 [H*3/2, W] buffer in cv2's layout `layout`: NV12 / NV21 -- H luma rows, then H/2
+        rows of interleaved chroma (U first for NV12, V first for NV21); I420 / YV12 -- H luma rows, then the U and V
+        planes (V first for YV12) with two chroma rows per buffer row.  The rows may be pitched (any row stride); an I420 /
+        YV12 buffer then has its chroma rows at half the luma pitch, and must have a column stride of 1 and an even row
+        stride.  Raises ValueError on what cannot be viewed so."""
+        if layout not in cls.LAYOUTS:
+            raise ValueError("YUV420.from_buffer: layout must be one of %s (got %r)" % ("/".join(cls.LAYOUTS), layout))
+        if not torch.is_tensor(t) or t.dtype != torch.uint8 or t.dim() != 2:
+            raise ValueError("YUV420.from_buffer: the buffer must be a uint8 [H*3/2, W] tensor")
+        rows, W = int(t.shape[0]), int(t.shape[1])
+        if rows % 3 or rows == 0 or W % 2 or W == 0:
+            raise ValueError("YUV420.from_buffer: a %dx%d buffer is not [H*3/2, W] with H, W even and positive" % (rows, W))
+        H = rows // 3 * 2
+        y = t[:H]
+        if layout in ("NV12", "NV21"):
+            a, b = t[H:, 0::2], t[H:, 1::2]
+            return cls(y, a, b) if layout == "NV12" else cls(y, b, a)
+        pitch, col = t.stride()
+        if col != 1 or pitch % 2 or pitch < W:
+            raise ValueError("YUV420.from_buffer: an %s buffer needs rows of contiguous bytes at an even pitch >= W (got "
+                             "strides %s)" % (layout, t.stride()))
+        first = t.storage_offset() + H * pitch
+        a = torch.as_strided(t, (H // 2, W // 2), (pitch // 2, 1), first)
+        b = torch.as_strided(t, (H // 2, W // 2), (pitch // 2, 1), first + H // 2 * (pitch // 2))
+        return cls(y, a, b) if layout == "I420" else cls(y, b, a)
+
+    @classmethod
+    def nv12(cls, y, uv):
+        """A frame from a luma tensor y [H, W] and an interleaved U, V chroma tensor uv, [H/2, W] or [H/2, W/2, 2], which
+        need not be adjacent to y (NVDEC surfaces).  Views, never copies."""
+        if not torch.is_tensor(uv) or uv.dim() not in (2, 3) or (uv.dim() == 3 and uv.shape[2] != 2):
+            raise ValueError("YUV420.nv12: uv must be a [H/2, W] or [H/2, W/2, 2] tensor")
+        if uv.dim() == 3:
+            return cls(y, uv[:, :, 0], uv[:, :, 1])
+        return cls(y, uv[:, 0::2], uv[:, 1::2])
+
+    def hw(self, what, index):
+        """(H, W) of a well-formed frame; ValueError naming image `index` otherwise."""
+        for name, p in zip("yuv", self):
+            if not torch.is_tensor(p) or p.dtype != torch.uint8 or p.dim() != 2:
+                raise ValueError("%s: image %d: YUV420 plane %s must be a 2-D uint8 tensor" % (what, index, name))
+        H, W = (int(s) for s in self.y.shape)
+        if H < 2 or W < 2 or H % 2 or W % 2:
+            raise ValueError("%s: image %d is a %dx%d YUV420 frame; 4:2:0 frames have even sides" % (what, index, H, W))
+        for name, p in zip("uv", self[1:]):
+            if tuple(p.shape) != (H // 2, W // 2):
+                raise ValueError("%s: image %d: YUV420 plane %s is %s, must be [%d, %d] for a %dx%d frame"
+                                 % (what, index, name, tuple(p.shape), H // 2, W // 2, H, W))
+        return H, W
+
+
+# What the images of a raw-photo call are (on_device): host arrays, CUDA BGR / RGB tensors or YUV420 frames.  One call or
+# stream takes one kind.  False / True keep on_device a truth value: whether the images are in device memory.
+HOST, TENSOR, FRAME = False, True, "YUV420"
+KIND_NAMES = {HOST: "a host image", TENSOR: "a CUDA tensor", FRAME: "a YUV420 frame"}
+
+
+def on_device(im, device, what, index, channels="BGR"):
+    """The kind of image `index` of a raw-photo call: HOST, TENSOR (a CUDA tensor) or FRAME (a YUV420 frame); a tensor or
+    every plane of a frame must be on the engine's `device`, and a frame converts to BGR, so channels must be "BGR" (dtype
+    and shape are frontend_plan's to check).  Anything else is a host image, CPU tensors included."""
+    if isinstance(im, YUV420):
+        for name, p in zip("yuv", im):
+            if not (torch.is_tensor(p) and p.is_cuda):
+                raise ValueError("%s: image %d: YUV420 plane %s is not a CUDA tensor; frames must be in device memory"
+                                 % (what, index, name))
+            if p.device != device:
+                raise ValueError("%s: image %d: YUV420 plane %s is on %s, the engine runs on %s" % (what, index, name, p.device,
+                                                                                                 device))
+        if channels != "BGR":
+            raise ValueError("%s: image %d is a YUV420 frame, which converts to BGR; channels=%r does not apply"
+                             % (what, index, channels))
+        return FRAME
     if not (torch.is_tensor(im) and im.is_cuda):
-        return False
+        return HOST
     if im.device != device:
         raise ValueError("%s: image %d is on %s, the engine runs on %s" % (what, index, im.device, device))
-    return True
+    return TENSOR
 
 
-def images_on_device(images, device, what):
-    """True when every image of a list call is a CUDA tensor, False when none is; a mixed list raises ValueError."""
-    kinds = [on_device(im, device, what, i) for i, im in enumerate(images)]
-    if any(kinds) and not all(kinds):
-        i = kinds.index(not kinds[0])
-        raise ValueError("%s: image %d is %s but image 0 is %s; one call takes host images or CUDA tensors, not both"
-                         % (what, i, *(("a CUDA tensor", "a host image") if kinds[i] else ("a host image", "a CUDA tensor"))))
-    return bool(kinds) and kinds[0]
+def mixed_kinds(what, index, kind, other, whose):
+    return ValueError("%s: image %d is %s but %s is %s; a call or stream takes one kind (host images, CUDA tensors or YUV420 "
+                      "frames), not both" % (what, index, KIND_NAMES[kind], whose, KIND_NAMES[other]))
+
+
+def images_on_device(images, device, what, channels="BGR"):
+    """The kind (on_device) of every image of a list call: HOST (False) when none is in device memory, TENSOR (True) or
+    FRAME; a list of more than one kind raises ValueError."""
+    kinds = [on_device(im, device, what, i, channels) for i, im in enumerate(images)]
+    for i, k in enumerate(kinds):
+        if k != kinds[0]:
+            raise mixed_kinds(what, i, k, kinds[0], "image 0")
+    return kinds[0] if kinds else HOST
 
 
 def strided_descriptor(address, nbytes, offset, strides, channels="BGR"):
@@ -1240,6 +1339,40 @@ def resize_strided(tensors, channels, fxy, dst_hw, dst, stream):
                                                 N.ptr(np.ascontiguousarray(fxy, np.float64)),
                                                 N.ptr(np.ascontiguousarray(dst_hw, np.int32)), B, N.ptr(dst),
                                                 int(dst.shape[1]), int(dst.shape[2]), stream), "ctpn_resize_linear_u8_strided")
+
+
+def yuv420_descriptor(frame):
+    """ctpn_resize_linear_u8_yuv420's descriptor of a YUV420 frame: per plane (Y, U, V) (allocation address, its bytes,
+    byte offset of sample (0, 0), (row, column) byte strides), from the planes' storages (uint8: elements are bytes)."""
+    out = []
+    for p in frame:
+        st = p.untyped_storage()
+        out.append((st.data_ptr(), st.nbytes(), p.storage_offset(), tuple(int(s) for s in p.stride())))
+    return out
+
+
+def resize_yuv420(frames, fxy, dst_hw, dst, stream):
+    """resize_im of YUV420 frames, converted as cv2.cvtColor converts them, into the uint8 canvas dst [B, H, W, 3]
+    (ctpn_resize_linear_u8_yuv420)."""
+    B = len(frames)
+    desc = [d for f in frames for d in yuv420_descriptor(f)]
+    addr = np.array([d[0] for d in desc], np.uint64)
+    nbytes = np.array([d[1] for d in desc], np.uint64)
+    offs = np.array([d[2] for d in desc], np.int64)
+    strides = np.array([d[3] for d in desc], np.int64)
+    hw = np.array([f.shape[:2] for f in frames], np.int32)
+    N.check(N.lib.ctpn_resize_linear_u8_yuv420(N.ptr(addr), N.ptr(nbytes), N.ptr(offs), N.ptr(strides), N.ptr(hw),
+                                               N.ptr(np.ascontiguousarray(fxy, np.float64)),
+                                               N.ptr(np.ascontiguousarray(dst_hw, np.int32)), B, N.ptr(dst),
+                                               int(dst.shape[1]), int(dst.shape[2]), stream), "ctpn_resize_linear_u8_yuv420")
+
+
+def resize_in_place(images, kind, channels, fxy, dst_hw, dst, stream):
+    """resize_im of images in device memory of one kind (on_device: TENSOR or FRAME), read in place, into dst."""
+    if kind == FRAME:
+        resize_yuv420(images, fxy, dst_hw, dst, stream)
+    else:
+        resize_strided(images, channels, fxy, dst_hw, dst, stream)
 
 
 # ---- streamed photos: the parts of Engine._stream that need no device ---------------------------------------------------
