@@ -29,6 +29,8 @@
  *                        TextDetector.detect, lib/text_connector/detectors.py:19-49; graph builder
  *                        text_proposal_graph_builder.py:6-78; chains other.py:16-29; line fitting
  *                        text_proposal_connector.py:21-64 and text_proposal_connector_oriented.py:24-105
+ *   ctpn_line_crop_widths_host / ctpn_line_crops_u8   the recognizer's line crops (cv2.warpAffine) a user would otherwise
+ *                        cut from draw_boxes' image on the host
  *   ctpn_bbox_overlaps_host / ctpn_bbox_intersections_host   lib/utils/bbox.pyx:15-55, :57-95 (Cython, CPU)
  *   ctpn_anchor_targets_host   lib/rpn_msr/anchor_target_layer_tf.py:78-175, :201 (tf.py_func body, network.py:225-243;
  *                        training only -- host code, as the reference's is)
@@ -341,6 +343,32 @@ int ctpn_text_filter_nms_host(const float *proposals, const float *scores, int n
                               int *num_keep);
 int ctpn_text_groups_host(const float *proposals, const float *scores, int m, int im_w, const float *cfg9, int *offsets,
                           int *members, int members_capacity, int *num_groups, int *num_members);
+
+/* ---- text-line crops (the input of a line recognizer) ----
+ * The crop of a line [x1,y1,x2,y2,x3,y3,x4,y4,score] (corners TL, TR, BL, BR, in the resize_im frame) at height hc
+ * (2 <= hc <= 256) is cv2.warpAffine(resized, Minv, (Wc, hc), INTER_LINEAR | WARP_INVERSE_MAP, BORDER_REPLICATE) with
+ *   len = sqrt((x2-x1)^2 + (y2-y1)^2), ht = sqrt((x3-x1)^2 + (y3-y1)^2), Wc = max(2, rint(hc * len / max(ht, 1)))
+ *   Minv = [[(x2-x1)/(Wc-1), (x3-x1)/(hc-1), x1], [(y2-y1)/(Wc-1), (y3-y1)/(hc-1), y1]]
+ * in float64 without FMA (csrc/crop.cuh: one definition for both entry points; oracle/crop.py).  BR is not used.
+ *
+ * ctpn_line_crop_widths_host: Wc of each of n HOST lines [n][9] -> widths[n].  CTPN_ERR_INVALID naming the line when a
+ *   width is not finite or exceeds 2^20.
+ * ctpn_line_crops_u8: the crops of a batch's lines, bit-identical to that warpAffine.  canvas: DEVICE uint8, image b's
+ *   (h, w) = im_hw[2b..2b+1] pixels (BGR) at canvas + b * batch_pitch + y * row_pitch + 3x.  lines: DEVICE float64
+ *   [batch][rows][9] (ctpn_text_lines' layout); image b's first num_lines[b] rows are cropped into out[b], a DEVICE uint8
+ *   [num_lines[b]][hc][max_width[b]][3]: columns at and past a line's Wc are written as 0.  max_width[b] must be at least
+ *   every Wc of the image (ctpn_line_crop_widths_host on the same lines); a line whose Wc the kernel finds larger, or not
+ *   finite, gets no pixels and sets status[b] (DEVICE, or host memory the device can write) to 1 -- status is written
+ *   for such images only, so one buffer can collect several launches.  Taps are clamped to the image, so no line value,
+ *   NaN included, makes the kernel read outside it.  im_hw, num_lines, max_width and out are HOST arrays (1 <= batch <=
+ *   64), validated before any CUDA call (CTPN_ERR_INVALID naming the image): hc range, 0 <= num_lines[b] <= rows, h, w
+ *   >= 1, 3w <= row_pitch and h * row_pitch <= batch_pitch, and where num_lines[b] > 0 a non-NULL out[b] and
+ *   2 <= max_width[b] <= 2^20, non-NULL canvas, lines and status.  Stream-ordered, no allocation, no synchronisation;
+ *   CTPN_ERR_NO_DEVICE without a GPU. */
+int ctpn_line_crop_widths_host(const double *lines, int n, int hc, int *widths);
+int ctpn_line_crops_u8(const void *canvas, long long batch_pitch, int row_pitch, const int *im_hw, const double *lines,
+                       int batch, int rows, int hc, const int *num_lines, const int *max_width, void *const *out, int *status,
+                       void *stream);
 
 /* ---- RPN training targets (host; SURVEY.md 8(f) rank 4) -------------------------------------------------------------
  * The reference computes these on the CPU once per training image; so does this library (plain C++, no device work).

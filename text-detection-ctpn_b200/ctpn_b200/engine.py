@@ -684,8 +684,8 @@ class Engine:
         before any device work."""
         out = [None] * len(images)
         rows = self.result_rows()
-        for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
-                                                                "rois_images", channels=channels):
+        for idxs, items, out_h, resized, _, _ in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
+                                                                      "rois_images", channels=channels):
             for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, len(idxs), rows))):
                 out[i] = (r, items[k].im_scale, items[k].f) + ((resized[k],) if return_resized else ())
         return out
@@ -694,7 +694,9 @@ class Engine:
         """The batches of rois_images / detect_lines_images.  Per ragged batch: front-end, network and proposal layer on the
         device (detect_packed's buffer), then after(packed, items) -- device work enqueued on the rois, returning the buffer
         to bring back (None: the packed rois themselves) -- and one D2H of that buffer.  Yields (input indices, their
-        FrontendSteps, the pinned host copy, the resize_im outputs or None); the pinned copy is reused by the next batch.
+        FrontendSteps, the pinned host copy, the resize_im outputs or None, the uint8 resize_im canvas, the device buffer
+        brought back); the pinned copy is reused by the next batch, and the canvas is rewritten by the next batch's work on
+        the current stream.
         Host images go up in one pinned H2D per batch; CUDA tensors (images_on_device) are read in place by
         ctpn_resize_linear_u8_strided."""
         if not 1 <= int(max_batch) <= 64:
@@ -753,7 +755,7 @@ class Engine:
             out_h.copy_(result, non_blocking=True)
             resized = [u8[k, :p.resized[0], :p.resized[1]].cpu().numpy() for k, p in enumerate(items)] if return_resized else None
             torch.cuda.current_stream().synchronize()              # also frees the pinned sources for the next batch
-            yield idxs, items, out_h, resized
+            yield idxs, items, out_h, resized, u8, result
 
     # ---- text lines on the device ----------------------------------------------------------
     @staticmethod
@@ -818,7 +820,7 @@ class Engine:
         return out
 
     def detect_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None, channels="BGR"):
+                            cfg=None, channels="BGR", crop_height=None):
         """ctpn() (demo.py:55-68 minus file I/O) for a list of raw HxWx3 uint8 BGR images of any sizes, all on the device:
         the batches of rois_images (same inputs and batching), then the text-line connector (text_lines) on each batch's
         rois, and one D2H per batch of the packed lines, counts and statuses.  Returns, in input order, (lines float64
@@ -826,20 +828,34 @@ class Engine:
         return_resized.  lines is bit-identical to TextDetector(native=True).detect(boxes, scores[:, None], resized.shape[:2])
         on detect_images' output for that image (mode "H" / "O" as cfg.TEST.DETECT_MODE; cfg: the 9 connector constants,
         None = text_connect_cfg's).  Raises CtpnError where that connector raises (a proposal outside the image width).
-        images and channels: as for rois_images (host images, or CUDA tensors read in place; BGR or RGB)."""
+        images and channels: as for rois_images (host images, or CUDA tensors read in place; BGR or RGB).
+
+        crop_height=Hc (2..256): each tuple becomes (lines, f, crops, widths) (plus resized): crops a CUDA uint8
+        [m, Hc, max(widths), 3] tensor whose crops[j, :, :widths[j]] is line j cut out of the resize_im output as a line
+        recognizer takes it -- cv2.warpAffine(resized, Minv, (widths[j], Hc), INTER_LINEAR | WARP_INVERSE_MAP,
+        BORDER_REPLICATE) with the map of include/ctpn_b200.h (ctpn_line_crops_u8), bit for bit -- and zeros past
+        widths[j]; widths an int64 array [m].  The crops are cut on the device from the canvas the lines were found on: no
+        image byte comes back for them and nothing goes up.  They are ready on the stream that was current when the call
+        was made."""
         if mode not in ("H", "O"):
             raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
+        check_crop_height(crop_height, "detect_lines_images")
         rows = self.result_rows()
+        stream = torch.cuda.current_stream()
 
         def connect(packed, items):
             return self._connect(packed, items, mode, cfg)
 
         out = [None] * len(images)
-        for idxs, items, out_h, resized in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
-                                                                "detect_lines_images", after=connect, channels=channels):
+        for idxs, items, out_h, resized, u8, res in self._images_batches(images, resize, max_batch, return_resized, scale,
+                                                                         max_scale, "detect_lines_images", after=connect,
+                                                                         channels=channels):
             per_image = self.split_lines(*self.unpack_lines(out_h.numpy(), len(idxs), rows), im_hw=[p.resized for p in items])
+            crops = [()] * len(idxs)
+            if crop_height is not None:     # before the next batch's front-end rewrites the canvas, in stream order
+                crops = self._line_crops(u8, res, items, per_image, crop_height, stream)
             for k, (i, lines) in enumerate(zip(idxs, per_image)):
-                out[i] = (lines, items[k].f) + ((resized[k],) if return_resized else ())
+                out[i] = (lines, items[k].f) + crops[k] + ((resized[k],) if return_resized else ())
         return out
 
     def detect_images(self, images, resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200, channels="BGR"):
@@ -872,7 +888,7 @@ class Engine:
         return buf
 
     def _stream(self, images, split, what, resize, max_batch, return_resized, scale, max_scale, window, compact_rows, after=None,
-                channels="BGR"):
+                channels="BGR", crop=None):
         """The generator behind stream_rois_images / stream_images / stream_lines_images: run_stream over the batches of
         stream_windows with these stages, on two slots used alternately --
           pack     (worker thread) the batch's rows, row maps, sizes and im_info into the slot's pinned buffer
@@ -882,7 +898,9 @@ class Engine:
           compute  on the current stream: the front-end kernels, detect_packed and after(packed, items), as _images_batches
                    runs them, into the slot's uint8 canvas; then on the result stream one D2H of the result (and, with
                    return_resized, one of the uint8 canvas);
-          finish   waits for that D2H and splits it: split(host buffer, batch) -> one tuple per image.
+          finish   waits for that D2H and splits it: split(host buffer, batch) -> one tuple per image; then, with crop,
+                   crop(tuples, batch, uint8 canvas, device result, compute stream) -> the tuples extended, enqueued on the
+                   compute stream before the next compute, which reuses the slot's canvas, is.
         The host blocks only in finish, for the batch it is about to yield.  A stream of CUDA tensors (its first image
         decides) packs and uploads the sizes and im_info only, and compute reads the tensors in place
         (ctpn_resize_linear_u8_strided); each batch holds its tensors until its results have come back."""
@@ -990,12 +1008,14 @@ class Engine:
                 returned[slot] = torch.cuda.Event()
                 returned[slot].record(result_stream)
             # the device results and the batch's input tensors live until the D2H, which follows the compute, has run
-            return out_h, res_h, returned[slot], (packed, result, batch.images)
+            return out_h, res_h, returned[slot], (packed, result, batch.images, u8)
 
         def finish(batch, handle):
-            out_h, res_h, ev, _keep = handle
+            out_h, res_h, ev, keep = handle
             ev.synchronize()
             per_image = split(out_h, batch)
+            if crop is not None:
+                per_image = crop(per_image, batch, keep[3], keep[1], main)
             if res_h is not None:
                 rn = res_h.numpy()
                 per_image = [t + (rn[k, :p.resized[0], :p.resized[1]].copy(),) for k, (t, p) in enumerate(zip(per_image, batch.items))]
@@ -1056,11 +1076,14 @@ class Engine:
                             compact_rows, channels=channels)
 
     def stream_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None, window=None, compact_rows=True, channels="BGR"):
+                            cfg=None, window=None, compact_rows=True, channels="BGR", crop_height=None):
         """detect_lines_images as a generator over any iterable of raw photos: see stream_rois_images; the connector runs
-        on each batch's rois on the device and only the lines come back.  Raises CtpnError where detect_lines_images does."""
+        on each batch's rois on the device and only the lines come back.  Raises CtpnError where detect_lines_images does.
+        crop_height: as for detect_lines_images; a batch's crops are cut when its lines have come back, before the canvas
+        is reused, on the stream that was current when the generator was created, and stay valid after it is closed."""
         if mode not in ("H", "O"):
             raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
+        check_crop_height(crop_height, "stream_lines_images")
         rows = self.result_rows()
 
         def split(out_h, batch):
@@ -1068,8 +1091,15 @@ class Engine:
             lines = self.split_lines(*self.unpack_lines(out_h.numpy(), len(hw), rows), im_hw=hw)
             return [(ln, p.f) for ln, p in zip(lines, batch.items)]
 
+        crop = None
+        if crop_height is not None:
+            def crop(per_image, batch, u8, res, stream):
+                crops = self._line_crops(u8, res, batch.items, [t[0] for t in per_image], crop_height, stream)
+                return [t + c for t, c in zip(per_image, crops)]
+
         return self._stream(images, split, "stream_lines_images", resize, max_batch, return_resized, scale, max_scale, window,
-                            compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg), channels=channels)
+                            compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg), channels=channels,
+                            crop=crop)
 
     def _connect(self, packed, items, mode, cfg):
         """The text-line connector on one batch's packed rois -> the packed lines (unpack_lines), on the device."""
@@ -1079,6 +1109,48 @@ class Engine:
         self.text_lines(rois, count, [p.resized for p in items], [p.im_scale for p in items], mode, cfg,
                         out=self.unpack_lines(res, B, rows))
         return res
+
+    def _line_crops(self, u8, res, items, lines, crop_height, stream):
+        """The line crops of one batch on `stream` (ctpn_line_crops_u8): u8 the batch's uint8 resize_im canvas [B, Hr, Wr, 3],
+        res its packed device lines (_connect), lines the same lines on the host, one float64 [m, 9] array per image.
+        Returns one (crops, widths) pair per image.  Each image's widths are computed on the host
+        (ctpn_line_crop_widths_host) and travel with the launch by value, with the output pointers.  The kernel recomputes
+        every width from the device lines; one that differs sets the image's entry of the engine's status array, which
+        this method checks at each call -- so such a fault, which one shared width definition rules out, is raised by the
+        next crop call that finds it."""
+        B, rows, hc = len(items), self.result_rows(), int(crop_height)
+        status = self._crop_status_buffer()
+        widths, crops = [], []
+        with torch.cuda.stream(stream):
+            for b, ln in enumerate(lines):
+                ln = np.ascontiguousarray(ln, np.float64)
+                w = np.zeros(len(ln), np.int32)
+                N.check(N.lib.ctpn_line_crop_widths_host(N.ptr(ln), len(ln), hc, N.ptr(w)),
+                        "ctpn_line_crop_widths_host (image %d of the batch)" % b)
+                widths.append(w.astype(np.int64))
+                crops.append(torch.empty((len(ln), hc, int(w.max()) if len(w) else 0, 3), dtype=torch.uint8,
+                                         device=self.device))
+            hw = np.array([p.resized for p in items], np.int32)
+            num = np.array([len(w) for w in widths], np.int32)
+            wmax = np.array([int(w.max()) if len(w) else 0 for w in widths], np.int32)
+            outs = np.array([c.data_ptr() for c in crops], np.uint64)
+            Hr, Wr = int(u8.shape[1]), int(u8.shape[2])
+            N.check(N.lib.ctpn_line_crops_u8(N.ptr(u8), Hr * Wr * 3, Wr * 3, N.ptr(hw), N.ptr(res), B, rows, hc,
+                                             N.ptr(num), N.ptr(wmax), N.ptr(outs), N.ptr(status), N.stream_ptr(stream)),
+                    "ctpn_line_crops_u8")
+        return [(c, w) for c, w in zip(crops, widths)]
+
+    def _crop_status_buffer(self):
+        """The engine's pinned int32 [64] crop status array, which the crop kernel writes through the unified address space
+        (no copy); raises CtpnError, and clears it, when an earlier launch has set an entry."""
+        st = getattr(self, "_crop_status", None)
+        if st is None:
+            st = self._crop_status = torch.zeros(64, dtype=torch.int32, pin_memory=True)
+        if bool(st.any()):
+            st.zero_()
+            raise N.CtpnError("ctpn_line_crops_u8: a line's crop width on the device differed from the host's; its crop was "
+                              "not written")
+        return st
 
     def detect(self, image, im_scale=1.0):
         """Single image [H,W,3] -> (scores, boxes); the test_ctpn() contract."""
@@ -1183,6 +1255,14 @@ def frontend_plan(shapes, resize=True, scale=600, max_scale=1200, cfg=None, firs
 
 # ---- photos already in device memory ------------------------------------------------------------------------------------
 CHANNELS = ("BGR", "RGB")
+
+
+def check_crop_height(crop_height, what):
+    """crop_height of the line calls: None (no crops) or an int 2..256."""
+    if crop_height is None:
+        return
+    if isinstance(crop_height, (bool, np.bool_)) or not isinstance(crop_height, (int, np.integer)) or not 2 <= crop_height <= 256:
+        raise ValueError("%s: crop_height must be None or an int 2..256 (got %r)" % (what, crop_height))
 
 
 def check_channels(channels, what):
