@@ -31,6 +31,7 @@
  *                        text_proposal_connector.py:21-64 and text_proposal_connector_oriented.py:24-105
  *   ctpn_line_crop_widths_host / ctpn_line_crops_u8   the recognizer's line crops (cv2.warpAffine) a user would otherwise
  *                        cut from draw_boxes' image on the host
+ *   ctpn_line_crops_strided_u8 / ctpn_line_crops_yuv420_u8   the same crops out of the source images at full resolution
  *   ctpn_bbox_overlaps_host / ctpn_bbox_intersections_host   lib/utils/bbox.pyx:15-55, :57-95 (Cython, CPU)
  *   ctpn_anchor_targets_host   lib/rpn_msr/anchor_target_layer_tf.py:78-175, :201 (tf.py_func body, network.py:225-243;
  *                        training only -- host code, as the reference's is)
@@ -364,11 +365,36 @@ int ctpn_text_groups_host(const float *proposals, const float *scores, int m, in
  *   64), validated before any CUDA call (CTPN_ERR_INVALID naming the image): hc range, 0 <= num_lines[b] <= rows, h, w
  *   >= 1, 3w <= row_pitch and h * row_pitch <= batch_pitch, and where num_lines[b] > 0 a non-NULL out[b] and
  *   2 <= max_width[b] <= 2^20, non-NULL canvas, lines and status.  Stream-ordered, no allocation, no synchronisation;
- *   CTPN_ERR_NO_DEVICE without a GPU. */
+ *   CTPN_ERR_NO_DEVICE without a GPU.
+ *
+ * Source crops: the same recipe applied to the SOURCE line of each line and the source image, at full resolution.  With
+ * f[b] the resize_im factor of image b, the source line is the line's corners divided by f[b], one IEEE float64 division
+ * each (src = line / f, as draw_boxes divides; numpy's lines[:, :8] / f on the host gives the same bits, and
+ * ctpn_line_crop_widths_host on those gives the widths), and the crop is cv2.warpAffine(source_bgr, Minv(src), ...).
+ * ctpn_line_crops_strided_u8: the sources are read in place, as ctpn_resize_linear_u8_strided reads them (src, src_bytes,
+ *   src_offset, src_strides, src_hw: its descriptors and its rules; a host image uploaded whole is the descriptor
+ *   (w * 3, 3, 1)).  At most 64 images, one launch.
+ * ctpn_line_crops_yuv420_u8: the sources are YUV 4:2:0 frames, described and checked as ctpn_resize_linear_u8_yuv420
+ *   describes them; each sample is converted as cv2.cvtColor(COLOR_YUV2BGR_*) converts it.  At most 64 frames, launched
+ *   in chunks of 32 (three planes' descriptors per frame).
+ * Both: lines DEVICE float64 [batch][rows][9] in the resize_im frame; num_lines, max_width, out and status as for
+ *   ctpn_line_crops_u8, with max_width[b] at least every source width of image b.  f, num_lines, max_width, out and the
+ *   descriptors are HOST arrays (1 <= batch <= 64), validated before any CUDA call (CTPN_ERR_INVALID naming the image, and
+ *   the plane): the hc range, 0 <= num_lines[b] <= rows, f[b] finite and > 0, the descriptor rules, where num_lines[b] > 0
+ *   a non-NULL out[b] and 2 <= max_width[b] <= 2^20, and non-NULL lines and status when any image has lines.  Taps are
+ *   clamped to the source image.  Stream-ordered, no allocation, no synchronisation; CTPN_ERR_NO_DEVICE without a GPU. */
 int ctpn_line_crop_widths_host(const double *lines, int n, int hc, int *widths);
 int ctpn_line_crops_u8(const void *canvas, long long batch_pitch, int row_pitch, const int *im_hw, const double *lines,
                        int batch, int rows, int hc, const int *num_lines, const int *max_width, void *const *out, int *status,
                        void *stream);
+int ctpn_line_crops_strided_u8(const void *const *src, const size_t *src_bytes, const long long *src_offset,
+                               const long long *src_strides, const int *src_hw, const double *f, const double *lines, int batch,
+                               int rows, int hc, const int *num_lines, const int *max_width, void *const *out, int *status,
+                               void *stream);
+int ctpn_line_crops_yuv420_u8(const void *const *planes, const size_t *plane_bytes, const long long *plane_offset,
+                              const long long *plane_strides, const int *src_hw, const double *f, const double *lines, int batch,
+                              int rows, int hc, const int *num_lines, const int *max_width, void *const *out, int *status,
+                              void *stream);
 
 /* ---- RPN training targets (host; SURVEY.md 8(f) rank 4) -------------------------------------------------------------
  * The reference computes these on the CPU once per training image; so does this library (plain C++, no device work).

@@ -1,5 +1,5 @@
-// The geometry of a text-line crop, ONE definition for the host widths (ctpn_line_crop_widths_host) and the crop kernel
-// (ctpn_line_crops_u8, crop.cu).  A line is a row [x1,y1,x2,y2,x3,y3,x4,y4,score] of the connector's output, corners TL,
+// The geometry of a text-line crop, ONE definition for the host widths (ctpn_line_crop_widths_host) and the crop kernels
+// (ctpn_line_crops_u8, ctpn_line_crops_strided_u8, ctpn_line_crops_yuv420_u8: crop.cu).  A line is a row [x1,y1,x2,y2,x3,y3,x4,y4,score] of the connector's output, corners TL,
 // TR, BL, BR; its crop of height hc is cv2.warpAffine of the resize_im output by the map below (oracle/crop.py):
 //   len = sqrt((x2-x1)^2 + (y2-y1)^2), ht = sqrt((x3-x1)^2 + (y3-y1)^2), Wc = max(2, rint(hc * len / max(ht, 1)))
 //   dst (0, 0) -> TL, (Wc-1, 0) -> TR, (0, hc-1) -> BL.
@@ -42,6 +42,19 @@ CROP_HD Map map(const double *ln, int wc, int hc) {
   a.m[4] = (ln[5] - ln[1]) / (double)(hc - 1);
   a.m[5] = ln[1];
   return a;
+}
+
+// The source line of a line of the resize_im frame at resize factor f: its corners divided by f, one IEEE float64 division
+// each -- the division draw_boxes makes, and numpy's lines[:, :8] / f on the host, bit for bit.  Only TL, TR and BL
+// (src[0..5]) enter the width and the map.
+CROP_HD void source_line(const double *ln, double f, double *src) {
+  for (int i = 0; i < 6; ++i) {
+#ifdef __CUDA_ARCH__
+    src[i] = __ddiv_rn(ln[i], f);
+#else
+    src[i] = ln[i] / f;
+#endif
+  }
 }
 
 }  // namespace crop

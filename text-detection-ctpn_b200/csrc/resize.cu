@@ -23,6 +23,7 @@
 // ctpn_resize_linear_u8_strided the ragged resize on images read in place at any byte strides (CUDA tensors of callers);
 // ctpn_resize_linear_u8_yuv420 converts YUV 4:2:0 frames read in place to BGR as cv2.cvtColor does, inside that resize.
 #include "common.cuh"
+#include "pixels.cuh"
 
 namespace ctpn {
 
@@ -61,40 +62,8 @@ struct CompactRows {
   }
   __device__ __forceinline__ uint8_t at(const uint8_t *r, int x, int c) const { return r[(size_t)x * C + c]; }
 };
-// ... or anywhere, at signed byte strides per row, column and channel (ctpn_resize_linear_u8_strided: a caller's device
-// tensor read in place; a negative channel stride from channel 2 reads RGB as BGR, a zero stride broadcasts).
-struct StridedPixels {
-  const uint8_t *base;         // sample (0, 0, 0)
-  long long row_stride;
-  int col_stride, chan_stride;
-  __device__ __forceinline__ const uint8_t *row(int y) const { return base + (long long)y * row_stride; }
-  __device__ __forceinline__ uint8_t at(const uint8_t *r, int x, int c) const {
-    return __ldg(r + ((long long)x * col_stride + (long long)c * chan_stride));
-  }
-};
-// ... or converted from YUV 4:2:0 planes on the fly (ctpn_resize_linear_u8_yuv420: video frames read in place), exactly as
-// cv2.cvtColor(COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) converts them: BT.601 limited range in 20-bit fixed point,
-// nearest chroma -- chroma sample (y >> 1, x >> 1) serves luma sample (y, x).  Every term fits in int32 and >> is
-// arithmetic, as in OpenCV's 4:2:0 converters (restated and pinned against cv2 in oracle/yuv.py).  The row handle is a
-// luma row plus the chroma rows of row >> 1; rows and columns come in clamped, so the chroma indices are in range too.
-struct Yuv420Pixels {
-  const uint8_t *y, *u, *v;    // sample (0, 0) of each plane
-  long long y_row, u_row, v_row;
-  int y_col, u_col, v_col;
-  struct Row {
-    const uint8_t *y, *u, *v;
-  };
-  __device__ __forceinline__ Row row(int r) const {
-    return Row{y + (long long)r * y_row, u + (long long)(r >> 1) * u_row, v + (long long)(r >> 1) * v_row};
-  }
-  __device__ __forceinline__ uint8_t at(const Row &r, int x, int c) const {
-    const int Y = __ldg(r.y + (long long)x * y_col);
-    const int U = __ldg(r.u + (long long)(x >> 1) * u_col) - 128, V = __ldg(r.v + (long long)(x >> 1) * v_col) - 128;
-    const int yy = max(Y - 16, 0) * 1220542 + (1 << 19);
-    const int t = c == 0 ? yy + 2116026 * U : c == 1 ? yy - 852492 * V - 409993 * U : yy + 1673527 * V;
-    return (uint8_t)min(max(t >> 20, 0), 255);
-  }
-};
+// ... or anywhere, at signed byte strides (StridedPixels: ctpn_resize_linear_u8_strided), or converted from YUV 4:2:0
+// planes on the fly (Yuv420Pixels: ctpn_resize_linear_u8_yuv420) -- pixels.cuh, shared with the line crops.
 
 // One output pixel of cv2.resize(INTER_LINEAR) of a uint8 image of sh x sw pixels and C channels -> o[C].  Shared by
 // every uint8 resize kernel: a ragged or strided batch is bit-identical to single-image runs by construction.  Taps,
@@ -526,29 +495,15 @@ extern "C" int ctpn_resize_linear_u8_strided(const void *const *src, const size_
   long long max_pixels = 0, work = 0;
   for (int b = 0; b < B; ++b) {
     const int sh = src_hw[2 * b], sw = src_hw[2 * b + 1];
-    CTPN_REQUIRE(src[b], "%s: image %d: null source", fn, b);
-    CTPN_REQUIRE(sh > 0 && sw > 0, "%s: image %d: bad source size %d x %d", fn, b, sh, sw);
-    const long long off = src_offset[b], *st = src_strides + 3 * b;
-    CTPN_REQUIRE(st[1] >= INT_MIN && st[1] <= INT_MAX && st[2] >= INT_MIN && st[2] <= INT_MAX,
-                 "%s: image %d: column / channel stride (%lld, %lld) outside the 32-bit range", fn, b, st[1], st[2]);
-    // lowest and highest byte of the h x w x 3 box, relative to the allocation; 128-bit, so no stride can wrap them
-    __int128 lo = off, hi = off;
-    const long long extent[3] = {sh - 1, sw - 1, 2};
-    for (int d = 0; d < 3; ++d) {
-      const __int128 span = (__int128)extent[d] * st[d];
-      (span < 0 ? lo : hi) += span;
-    }
-    CTPN_REQUIRE(lo >= 0 && hi < (__int128)src_bytes[b],
-                 "%s: image %d: the box spans bytes [%lld, %lld] of its allocation, outside [0, %zu)", fn, b,
-                 (long long)std::max<__int128>(std::min<__int128>(lo, LLONG_MAX), LLONG_MIN),
-                 (long long)std::max<__int128>(std::min<__int128>(hi, LLONG_MAX), LLONG_MIN), src_bytes[b]);
-    int eh = 0, ew = 0;
-    const int rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew);
+    StridedPixels px;
+    int rc = strided_source(fn, b, src[b], src_bytes[b], src_offset[b], src_strides + 3 * b, sh, sw, &px);
     if (rc) return rc;
-    p.base[b] = (const uint8_t *)src[b] + off;
-    p.row_stride[b] = st[0];
-    p.col_stride[b] = (int)st[1];
-    p.chan_stride[b] = (int)st[2];
+    int eh = 0, ew = 0;
+    if ((rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew))) return rc;
+    p.base[b] = px.base;
+    p.row_stride[b] = px.row_stride;
+    p.col_stride[b] = px.col_stride;
+    p.chan_stride[b] = px.chan_stride;
     p.sh[b] = sh;
     p.sw[b] = sw;
     p.dh[b] = eh;
@@ -572,7 +527,6 @@ extern "C" int ctpn_resize_linear_u8_yuv420(const void *const *planes, const siz
                                             const long long *plane_strides, const int *src_hw, const double *fxy,
                                             const int *dst_hw, int B, void *dst, int H, int W, void *stream) {
   const char *fn = "ctpn_resize_linear_u8_yuv420";
-  static const char *const kPlane[3] = {"Y", "U", "V"};
   CTPN_REQUIRE(dst, "%s: null pointer", fn);
   CTPN_REQUIRE(planes && plane_bytes && plane_offset && plane_strides && src_hw && fxy && dst_hw, "%s: null descriptor array",
                fn);
@@ -583,34 +537,21 @@ extern "C" int ctpn_resize_linear_u8_yuv420(const void *const *planes, const siz
   long long max_pixels[(kRaggedMax + kYuvChunk - 1) / kYuvChunk] = {}, work = 0;
   for (int b = 0; b < B; ++b) {
     const int sh = src_hw[2 * b], sw = src_hw[2 * b + 1];
-    CTPN_REQUIRE(sh > 0 && sw > 0 && sh % 2 == 0 && sw % 2 == 0, "%s: image %d: source size %d x %d must be even and positive",
-                 fn, b, sh, sw);
+    Yuv420Pixels px;
+    int rc = yuv420_source(fn, b, planes + 3 * b, plane_bytes + 3 * b, plane_offset + 3 * b, plane_strides + 6 * b, sh, sw, &px);
+    if (rc) return rc;
     Yuv420Resize &p = chunk[b / kYuvChunk];
     const int k = b % kYuvChunk;
+    const uint8_t *const pl[3] = {px.y, px.u, px.v};
+    const long long rs[3] = {px.y_row, px.u_row, px.v_row};
+    const int cs[3] = {px.y_col, px.u_col, px.v_col};
     for (int q = 0; q < 3; ++q) {
-      const int i = 3 * b + q;
-      const long long off = plane_offset[i], *st = plane_strides + 2 * i;
-      CTPN_REQUIRE(planes[i], "%s: image %d: null %s plane", fn, b, kPlane[q]);
-      CTPN_REQUIRE(st[1] >= INT_MIN && st[1] <= INT_MAX, "%s: image %d: %s plane column stride %lld outside the 32-bit range",
-                   fn, b, kPlane[q], st[1]);
-      // lowest and highest byte of the plane's box (h x w luma, h/2 x w/2 chroma); 128-bit, so no stride can wrap them
-      __int128 lo = off, hi = off;
-      const long long extent[2] = {(q ? sh / 2 : sh) - 1, (q ? sw / 2 : sw) - 1};
-      for (int d = 0; d < 2; ++d) {
-        const __int128 span = (__int128)extent[d] * st[d];
-        (span < 0 ? lo : hi) += span;
-      }
-      CTPN_REQUIRE(lo >= 0 && hi < (__int128)plane_bytes[i],
-                   "%s: image %d: the %s plane spans bytes [%lld, %lld] of its allocation, outside [0, %zu)", fn, b, kPlane[q],
-                   (long long)std::max<__int128>(std::min<__int128>(lo, LLONG_MAX), LLONG_MIN),
-                   (long long)std::max<__int128>(std::min<__int128>(hi, LLONG_MAX), LLONG_MIN), plane_bytes[i]);
-      p.plane[k][q] = (const uint8_t *)planes[i] + off;
-      p.row_stride[k][q] = st[0];
-      p.col_stride[k][q] = (int)st[1];
+      p.plane[k][q] = pl[q];
+      p.row_stride[k][q] = rs[q];
+      p.col_stride[k][q] = cs[q];
     }
     int eh = 0, ew = 0;
-    const int rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew);
-    if (rc) return rc;
+    if ((rc = ragged_geometry_ok(fn, b, sh, sw, fxy[2 * b], fxy[2 * b + 1], dst_hw, H, W, &eh, &ew))) return rc;
     p.H = H;
     p.W = W;
     p.sh[k] = sh;

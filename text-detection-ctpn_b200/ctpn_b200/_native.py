@@ -51,6 +51,8 @@ SIGNATURES = {
     "ctpn_text_groups_host": (_i, [_p, _p, _i, _i, _p, _p, _p, _i, _p, _p]),
     "ctpn_line_crop_widths_host": (_i, [_p, _i, _i, _p]),
     "ctpn_line_crops_u8": (_i, [_p, C.c_longlong, _i, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "ctpn_line_crops_strided_u8": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
+    "ctpn_line_crops_yuv420_u8": (_i, [_p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _p, _p, _p]),
     "ctpn_bbox_overlaps_host": (_i, [_p, _i, _i, _p, _i, _i, _p]),
     "ctpn_bbox_intersections_host": (_i, [_p, _i, _i, _p, _i, _i, _p]),
     "ctpn_anchor_targets_host": (_i, [_p, _i, _i, _p, _p, _i, _i, _i, _i, C.c_double, C.c_double, _p, _p, _p]),

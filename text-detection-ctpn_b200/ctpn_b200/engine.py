@@ -22,6 +22,7 @@ measured; activation scales calibrated on the first batch).
 """
 import collections
 import ctypes as C
+import functools
 
 import os
 
@@ -684,8 +685,8 @@ class Engine:
         before any device work."""
         out = [None] * len(images)
         rows = self.result_rows()
-        for idxs, items, out_h, resized, _, _ in self._images_batches(images, resize, max_batch, return_resized, scale, max_scale,
-                                                                      "rois_images", channels=channels):
+        for idxs, items, out_h, resized, _, _, _ in self._images_batches(images, resize, max_batch, return_resized, scale,
+                                                                         max_scale, "rois_images", channels=channels):
             for k, (i, r) in enumerate(zip(idxs, self._split_results(out_h, len(idxs), rows))):
                 out[i] = (r, items[k].im_scale, items[k].f) + ((resized[k],) if return_resized else ())
         return out
@@ -695,8 +696,9 @@ class Engine:
         device (detect_packed's buffer), then after(packed, items) -- device work enqueued on the rois, returning the buffer
         to bring back (None: the packed rois themselves) -- and one D2H of that buffer.  Yields (input indices, their
         FrontendSteps, the pinned host copy, the resize_im outputs or None, the uint8 resize_im canvas, the device buffer
-        brought back); the pinned copy is reused by the next batch, and the canvas is rewritten by the next batch's work on
-        the current stream.
+        brought back, a callable giving the batch's sources for source crops (line_crop_sources)); the pinned copy is reused
+        by the next batch, and the canvas and the uploaded sources are rewritten by the next batch's work on the current
+        stream.
         Host images go up in one pinned H2D per batch; CUDA tensors (images_on_device) are read in place by
         ctpn_resize_linear_u8_strided."""
         if not 1 <= int(max_batch) <= 64:
@@ -722,8 +724,10 @@ class Engine:
                 canvas = torch.empty((B, H, W, 3), dtype=torch.float32, device=self.device)
             resized_hw = np.array([p.resized for p in items], np.int32)
             fxy = np.array([[p.f, p.f] for p in items], np.float64)
+            batch_images = [images[i] for i in idxs]
             if device_images:      # read in place: no staging, no image H2D
-                resize_in_place([images[i] for i in idxs], device_images, channels, fxy, resized_hw, u8, stream)
+                resize_in_place(batch_images, device_images, channels, fxy, resized_hw, u8, stream)
+                sources = functools.partial(line_crop_sources, batch_images, device_images, channels)
             else:
                 nbytes = [images[i].size for i in idxs]
                 offsets = np.cumsum([0] + nbytes[:-1]).astype(np.int64)
@@ -739,6 +743,7 @@ class Engine:
                 N.check(N.lib.ctpn_resize_linear_u8_ragged(N.ptr(src), total, N.ptr(offsets), N.ptr(hwp), N.ptr(fxy),
                                                            N.ptr(resized_hw), B, 3, N.ptr(u8), Hr, Wr, stream),
                         "ctpn_resize_linear_u8_ragged")
+                sources = functools.partial(line_crop_sources, batch_images, HOST, "BGR", src, offsets)
             if not is_u8:
                 boffs = np.arange(B, dtype=np.int64) * (Hr * Wr * 3)
                 bhwp = np.concatenate([resized_hw, np.full((B, 1), Wr, np.int32)], axis=1)
@@ -755,7 +760,7 @@ class Engine:
             out_h.copy_(result, non_blocking=True)
             resized = [u8[k, :p.resized[0], :p.resized[1]].cpu().numpy() for k, p in enumerate(items)] if return_resized else None
             torch.cuda.current_stream().synchronize()              # also frees the pinned sources for the next batch
-            yield idxs, items, out_h, resized, u8, result
+            yield idxs, items, out_h, resized, u8, result, sources
 
     # ---- text lines on the device ----------------------------------------------------------
     @staticmethod
@@ -820,7 +825,7 @@ class Engine:
         return out
 
     def detect_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None, channels="BGR", crop_height=None):
+                            cfg=None, channels="BGR", crop_height=None, crop_from="resized"):
         """ctpn() (demo.py:55-68 minus file I/O) for a list of raw HxWx3 uint8 BGR images of any sizes, all on the device:
         the batches of rois_images (same inputs and batching), then the text-line connector (text_lines) on each batch's
         rois, and one D2H per batch of the packed lines, counts and statuses.  Returns, in input order, (lines float64
@@ -836,10 +841,20 @@ class Engine:
         BORDER_REPLICATE) with the map of include/ctpn_b200.h (ctpn_line_crops_u8), bit for bit -- and zeros past
         widths[j]; widths an int64 array [m].  The crops are cut on the device from the canvas the lines were found on: no
         image byte comes back for them and nothing goes up.  They are ready on the stream that was current when the call
-        was made."""
+        was made.
+
+        crop_from="source" (with crop_height): the crops are cut out of the source photo at full resolution instead of the
+        resize_im canvas -- crops[j, :, :widths[j]] is the same recipe applied to the source line lines[j, :8] / f (float64,
+        the division draw_boxes makes) and the source image in BGR: a host image as passed (flipped with channels="RGB"),
+        a tensor read through its strides, a YUV420 frame as cv2.cvtColor converts it (ctpn_line_crops_strided_u8 /
+        ctpn_line_crops_yuv420_u8).  The lines stay in the resize_im frame; widths are the source widths.  The sources are
+        read where they already are on the device -- host images in the batch's upload, tensors and frames in place -- so
+        nothing more crosses the bus.  With f = 1 (resize=False, or a photo already at `scale`) both settings give the
+        same crops.  crop_from="resized" (default) is the canvas crop above."""
         if mode not in ("H", "O"):
             raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
         check_crop_height(crop_height, "detect_lines_images")
+        check_crop_from(crop_from, crop_height, "detect_lines_images")
         rows = self.result_rows()
         stream = torch.cuda.current_stream()
 
@@ -847,13 +862,14 @@ class Engine:
             return self._connect(packed, items, mode, cfg)
 
         out = [None] * len(images)
-        for idxs, items, out_h, resized, u8, res in self._images_batches(images, resize, max_batch, return_resized, scale,
-                                                                         max_scale, "detect_lines_images", after=connect,
-                                                                         channels=channels):
+        for idxs, items, out_h, resized, u8, res, sources in self._images_batches(images, resize, max_batch, return_resized,
+                                                                                  scale, max_scale, "detect_lines_images",
+                                                                                  after=connect, channels=channels):
             per_image = self.split_lines(*self.unpack_lines(out_h.numpy(), len(idxs), rows), im_hw=[p.resized for p in items])
             crops = [()] * len(idxs)
-            if crop_height is not None:     # before the next batch's front-end rewrites the canvas, in stream order
-                crops = self._line_crops(u8, res, items, per_image, crop_height, stream)
+            if crop_height is not None:     # before the next batch's front-end rewrites the canvas and sources, in stream order
+                crops = self._line_crops(u8, res, items, per_image, crop_height, stream,
+                                         sources() if crop_from == "source" else None)
             for k, (i, lines) in enumerate(zip(idxs, per_image)):
                 out[i] = (lines, items[k].f) + crops[k] + ((resized[k],) if return_resized else ())
         return out
@@ -888,7 +904,7 @@ class Engine:
         return buf
 
     def _stream(self, images, split, what, resize, max_batch, return_resized, scale, max_scale, window, compact_rows, after=None,
-                channels="BGR", crop=None):
+                channels="BGR", crop=None, source_crops=False):
         """The generator behind stream_rois_images / stream_images / stream_lines_images: run_stream over the batches of
         stream_windows with these stages, on two slots used alternately --
           pack     (worker thread) the batch's rows, row maps, sizes and im_info into the slot's pinned buffer
@@ -899,8 +915,13 @@ class Engine:
                    runs them, into the slot's uint8 canvas; then on the result stream one D2H of the result (and, with
                    return_resized, one of the uint8 canvas);
           finish   waits for that D2H and splits it: split(host buffer, batch) -> one tuple per image; then, with crop,
-                   crop(tuples, batch, uint8 canvas, device result, compute stream) -> the tuples extended, enqueued on the
-                   compute stream before the next compute, which reuses the slot's canvas, is.
+                   crop(tuples, batch, uint8 canvas, device result, compute stream, sources) -> the tuples extended, enqueued
+                   on the compute stream before the next compute, which reuses the slot's canvas, is.
+        source_crops (crop reads the sources, line_crop_sources): host images are uploaded whole (a line may lie on any
+        row, so compact_rows does not apply), into a ring of three device buffers indexed by batch number: the crop of
+        batch k - 1 is enqueued after upload(k + 1), so with two buffers that upload would overwrite its pixels; upload
+        (k + 1) reuses the buffer of batch k - 2 once that batch's crop has run.  Tensors and frames are recorded on the
+        compute stream after their crop, so their memory outlives it whatever the caller drops.
         The host blocks only in finish, for the batch it is about to yield.  A stream of CUDA tensors (its first image
         decides) packs and uploads the sizes and im_info only, and compute reads the tensors in place
         (ctpn_resize_linear_u8_strided); each batch holds its tensors until its results have come back."""
@@ -917,6 +938,9 @@ class Engine:
         main = torch.cuda.current_stream()
         lut = self._mean_lut()
         copied, computed, returned = [None, None], [None, None], [None, None]     # per slot: events of its last H2D / compute / D2H
+        cropped, uploads = [None] * 3, [0]     # source crops: per ring buffer, the event after the last crop that read it
+        if source_crops:
+            compact_rows = False
 
         device_images = []                      # [the kind (on_device) of the stream's images], set by its first image
 
@@ -943,17 +967,20 @@ class Engine:
 
         def upload(batch, slot, packed):
             lay, pinned = packed
-            dev = self._stream_buffer("src", slot, lay.total, copy_stream)
+            ring = uploads[0] % 3 if source_crops else slot
+            uploads[0] += 1
+            free = cropped[ring] if source_crops else computed[slot]
+            dev = self._stream_buffer("src", ring, lay.total, copy_stream)
             with torch.cuda.stream(copy_stream):
-                if computed[slot] is not None:
-                    copy_stream.wait_event(computed[slot])
+                if free is not None:
+                    copy_stream.wait_event(free)
                 dev[:lay.total].copy_(pinned[:lay.total], non_blocking=True)          # the batch's one H2D
                 copied[slot] = torch.cuda.Event()
                 copied[slot].record(copy_stream)
-            return lay, dev, copied[slot]
+            return lay, dev, copied[slot], ring
 
         def compute(batch, slot, uploaded):
-            lay, dev, arrived = uploaded
+            lay, dev, arrived, ring = uploaded
             items, (H, W) = batch.items, batch.canvas
             B = len(items)
             stream = N.stream_ptr()
@@ -1008,14 +1035,24 @@ class Engine:
                 returned[slot] = torch.cuda.Event()
                 returned[slot].record(result_stream)
             # the device results and the batch's input tensors live until the D2H, which follows the compute, has run
-            return out_h, res_h, returned[slot], (packed, result, batch.images, u8)
+            return out_h, res_h, returned[slot], (packed, result, batch.images, u8, lay, dev, ring)
 
         def finish(batch, handle):
             out_h, res_h, ev, keep = handle
             ev.synchronize()
             per_image = split(out_h, batch)
             if crop is not None:
-                per_image = crop(per_image, batch, keep[3], keep[1], main)
+                lay, dev, ring = keep[4:]
+                sources = None
+                if source_crops:
+                    sources = line_crop_sources(batch.images, device_images[0], channels, dev, lay.offsets)
+                per_image = crop(per_image, batch, keep[3], keep[1], main, sources)
+                if source_crops:
+                    cropped[ring] = torch.cuda.Event()
+                    cropped[ring].record(main)
+                    for t in batch.images if device_images[0] else ():
+                        for p in (t if device_images[0] == FRAME else (t,)):
+                            p.record_stream(main)
             if res_h is not None:
                 rn = res_h.numpy()
                 per_image = [t + (rn[k, :p.resized[0], :p.resized[1]].copy(),) for k, (t, p) in enumerate(zip(per_image, batch.items))]
@@ -1076,14 +1113,18 @@ class Engine:
                             compact_rows, channels=channels)
 
     def stream_lines_images(self, images, mode="H", resize=True, max_batch=32, return_resized=False, scale=600, max_scale=1200,
-                            cfg=None, window=None, compact_rows=True, channels="BGR", crop_height=None):
+                            cfg=None, window=None, compact_rows=True, channels="BGR", crop_height=None, crop_from="resized"):
         """detect_lines_images as a generator over any iterable of raw photos: see stream_rois_images; the connector runs
         on each batch's rois on the device and only the lines come back.  Raises CtpnError where detect_lines_images does.
         crop_height: as for detect_lines_images; a batch's crops are cut when its lines have come back, before the canvas
-        is reused, on the stream that was current when the generator was created, and stay valid after it is closed."""
+        is reused, on the stream that was current when the generator was created, and stay valid after it is closed.
+        crop_from="source": as for detect_lines_images.  Host photos are then uploaded whole, whatever compact_rows says
+        (a line may lie on any source row, and its rows are known only once the lines are back), and the stream reads
+        tensors and frames until their crops have run, which are enqueued before their results are yielded."""
         if mode not in ("H", "O"):
             raise ValueError("mode must be 'H' or 'O' (got %r)" % (mode,))
         check_crop_height(crop_height, "stream_lines_images")
+        check_crop_from(crop_from, crop_height, "stream_lines_images")
         rows = self.result_rows()
 
         def split(out_h, batch):
@@ -1093,13 +1134,13 @@ class Engine:
 
         crop = None
         if crop_height is not None:
-            def crop(per_image, batch, u8, res, stream):
-                crops = self._line_crops(u8, res, batch.items, [t[0] for t in per_image], crop_height, stream)
+            def crop(per_image, batch, u8, res, stream, sources):
+                crops = self._line_crops(u8, res, batch.items, [t[0] for t in per_image], crop_height, stream, sources)
                 return [t + c for t, c in zip(per_image, crops)]
 
         return self._stream(images, split, "stream_lines_images", resize, max_batch, return_resized, scale, max_scale, window,
                             compact_rows, after=lambda packed, items: self._connect(packed, items, mode, cfg), channels=channels,
-                            crop=crop)
+                            crop=crop, source_crops=crop_from == "source")
 
     def _connect(self, packed, items, mode, cfg):
         """The text-line connector on one batch's packed rois -> the packed lines (unpack_lines), on the device."""
@@ -1110,9 +1151,11 @@ class Engine:
                         out=self.unpack_lines(res, B, rows))
         return res
 
-    def _line_crops(self, u8, res, items, lines, crop_height, stream):
+    def _line_crops(self, u8, res, items, lines, crop_height, stream, sources=None):
         """The line crops of one batch on `stream` (ctpn_line_crops_u8): u8 the batch's uint8 resize_im canvas [B, Hr, Wr, 3],
         res its packed device lines (_connect), lines the same lines on the host, one float64 [m, 9] array per image.
+        sources (line_crop_sources): cut from the batch's source images instead (ctpn_line_crops_strided_u8 /
+        ctpn_line_crops_yuv420_u8), at the source widths -- of lines / f, divided here as the kernel divides them.
         Returns one (crops, widths) pair per image.  Each image's widths are computed on the host
         (ctpn_line_crop_widths_host) and travel with the launch by value, with the output pointers.  The kernel recomputes
         every width from the device lines; one that differs sets the image's entry of the engine's status array, which
@@ -1123,7 +1166,9 @@ class Engine:
         widths, crops = [], []
         with torch.cuda.stream(stream):
             for b, ln in enumerate(lines):
-                ln = np.ascontiguousarray(ln, np.float64)
+                ln = np.array(ln, np.float64)
+                if sources is not None:
+                    ln[:, :8] /= np.float64(items[b].f)
                 w = np.zeros(len(ln), np.int32)
                 N.check(N.lib.ctpn_line_crop_widths_host(N.ptr(ln), len(ln), hc, N.ptr(w)),
                         "ctpn_line_crop_widths_host (image %d of the batch)" % b)
@@ -1134,10 +1179,19 @@ class Engine:
             num = np.array([len(w) for w in widths], np.int32)
             wmax = np.array([int(w.max()) if len(w) else 0 for w in widths], np.int32)
             outs = np.array([c.data_ptr() for c in crops], np.uint64)
-            Hr, Wr = int(u8.shape[1]), int(u8.shape[2])
-            N.check(N.lib.ctpn_line_crops_u8(N.ptr(u8), Hr * Wr * 3, Wr * 3, N.ptr(hw), N.ptr(res), B, rows, hc,
-                                             N.ptr(num), N.ptr(wmax), N.ptr(outs), N.ptr(status), N.stream_ptr(stream)),
-                    "ctpn_line_crops_u8")
+            if sources is None:
+                Hr, Wr = int(u8.shape[1]), int(u8.shape[2])
+                N.check(N.lib.ctpn_line_crops_u8(N.ptr(u8), Hr * Wr * 3, Wr * 3, N.ptr(hw), N.ptr(res), B, rows, hc,
+                                                 N.ptr(num), N.ptr(wmax), N.ptr(outs), N.ptr(status), N.stream_ptr(stream)),
+                        "ctpn_line_crops_u8")
+            else:
+                yuv, desc, src_hw = sources
+                name = "ctpn_line_crops_yuv420_u8" if yuv else "ctpn_line_crops_strided_u8"
+                addr, nbytes, offs, strides = descriptor_arrays(desc)
+                f = np.array([p.f for p in items], np.float64)
+                N.check(getattr(N.lib, name)(N.ptr(addr), N.ptr(nbytes), N.ptr(offs), N.ptr(strides), N.ptr(src_hw), N.ptr(f),
+                                             N.ptr(res), B, rows, hc, N.ptr(num), N.ptr(wmax), N.ptr(outs), N.ptr(status),
+                                             N.stream_ptr(stream)), name)
         return [(c, w) for c, w in zip(crops, widths)]
 
     def _crop_status_buffer(self):
@@ -1263,6 +1317,18 @@ def check_crop_height(crop_height, what):
         return
     if isinstance(crop_height, (bool, np.bool_)) or not isinstance(crop_height, (int, np.integer)) or not 2 <= crop_height <= 256:
         raise ValueError("%s: crop_height must be None or an int 2..256 (got %r)" % (what, crop_height))
+
+
+CROP_FROM = ("resized", "source")
+
+
+def check_crop_from(crop_from, crop_height, what):
+    """crop_from of the line calls: "resized" (crops out of the resize_im canvas) or "source" (out of the source images),
+    the latter only with a crop_height."""
+    if not isinstance(crop_from, str) or crop_from not in CROP_FROM:
+        raise ValueError("%s: crop_from must be 'resized' or 'source' (got %r)" % (what, crop_from))
+    if crop_from == "source" and crop_height is None:
+        raise ValueError("%s: crop_from='source' needs a crop_height" % what)
 
 
 def check_channels(channels, what):
@@ -1405,15 +1471,17 @@ def tensor_descriptor(t, channels="BGR"):
     return strided_descriptor(st.data_ptr(), st.nbytes(), t.storage_offset(), t.stride(), channels)
 
 
+def descriptor_arrays(desc):
+    """The host arrays (addresses, bytes, offsets, strides) of a list of strided_descriptor / yuv420_descriptor tuples."""
+    return (np.array([d[0] for d in desc], np.uint64), np.array([d[1] for d in desc], np.uint64),
+            np.array([d[2] for d in desc], np.int64), np.array([d[3] for d in desc], np.int64))
+
+
 def resize_strided(tensors, channels, fxy, dst_hw, dst, stream):
     """resize_im of CUDA uint8 [h, w, 3] tensors read in place into the uint8 canvas dst [B, H, W, 3]
     (ctpn_resize_linear_u8_strided)."""
     B = len(tensors)
-    desc = [tensor_descriptor(t, channels) for t in tensors]
-    addr = np.array([d[0] for d in desc], np.uint64)
-    nbytes = np.array([d[1] for d in desc], np.uint64)
-    offs = np.array([d[2] for d in desc], np.int64)
-    strides = np.array([d[3] for d in desc], np.int64)
+    addr, nbytes, offs, strides = descriptor_arrays([tensor_descriptor(t, channels) for t in tensors])
     hw = np.array([tuple(t.shape[:2]) for t in tensors], np.int32)
     N.check(N.lib.ctpn_resize_linear_u8_strided(N.ptr(addr), N.ptr(nbytes), N.ptr(offs), N.ptr(strides), N.ptr(hw),
                                                 N.ptr(np.ascontiguousarray(fxy, np.float64)),
@@ -1435,11 +1503,7 @@ def resize_yuv420(frames, fxy, dst_hw, dst, stream):
     """resize_im of YUV420 frames, converted as cv2.cvtColor converts them, into the uint8 canvas dst [B, H, W, 3]
     (ctpn_resize_linear_u8_yuv420)."""
     B = len(frames)
-    desc = [d for f in frames for d in yuv420_descriptor(f)]
-    addr = np.array([d[0] for d in desc], np.uint64)
-    nbytes = np.array([d[1] for d in desc], np.uint64)
-    offs = np.array([d[2] for d in desc], np.int64)
-    strides = np.array([d[3] for d in desc], np.int64)
+    addr, nbytes, offs, strides = descriptor_arrays([d for f in frames for d in yuv420_descriptor(f)])
     hw = np.array([f.shape[:2] for f in frames], np.int32)
     N.check(N.lib.ctpn_resize_linear_u8_yuv420(N.ptr(addr), N.ptr(nbytes), N.ptr(offs), N.ptr(strides), N.ptr(hw),
                                                N.ptr(np.ascontiguousarray(fxy, np.float64)),
@@ -1453,6 +1517,19 @@ def resize_in_place(images, kind, channels, fxy, dst_hw, dst, stream):
         resize_yuv420(images, fxy, dst_hw, dst, stream)
     else:
         resize_strided(images, channels, fxy, dst_hw, dst, stream)
+
+
+def line_crop_sources(images, kind, channels, buf=None, offsets=None):
+    """The sources of a batch's source crops: (is YUV, descriptors, int32 [B, 2] source sizes) for
+    ctpn_line_crops_strided_u8 / ctpn_line_crops_yuv420_u8.  Tensors and frames (kind TENSOR / FRAME) are read in place;
+    host images (HOST) are read where their upload put them: whole, BGR, each at byte offsets[b] of the device buffer buf."""
+    hw = np.array([tuple(im.shape[:2]) for im in images], np.int32).reshape(-1, 2)
+    if kind == FRAME:
+        return True, [d for f in images for d in yuv420_descriptor(f)], hw
+    if kind == HOST:
+        return False, [strided_descriptor(buf.data_ptr(), buf.numel(), int(o), (int(w) * 3, 3, 1))
+                       for o, (h, w) in zip(offsets, hw)], hw
+    return False, [tensor_descriptor(t, channels) for t in images], hw
 
 
 # ---- streamed photos: the parts of Engine._stream that need no device ---------------------------------------------------
